@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""Headline benchmark: Taylor steps/s (fp64, batch) of outer_ss_long_term_batch on N B200s.
+"""Headline benchmark: Taylor steps/s (fp64, batch) of outer_ss_long_term_batch on N H100s.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--dump-outputs DIR]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N ... bench.py --gpus N ...
 
 Workload (BASELINE.json configs[1]): the 6-body outer Solar System of benchmark/outer_ss_long_term_batch.cpp
@@ -13,14 +13,20 @@ n_steps field of get_propagate_res()) per second, whole job.
 Printed JSON line (see the task contract): value = device-timed whole-job throughput with inputs resident in
 HBM; e2e = the same through the host-buffer API (H2D of state/time/t_final from pinned memory + D2H of the
 final state and results inside the timed region); roofline = algorithmic bytes (B_tape of SURVEY.md 8(d)) /
-propagate-kernel time vs the measured HBM copy bandwidth; cpu_baseline = the oracle's 8-lane CPU port on all
-host cores on a bounded sample of the same workload.
+propagate-kernel time vs the HBM bandwidth; cpu_baseline = the oracle's 8-lane CPU port on all host cores on a
+bounded sample of the same workload.
+
+--dump-outputs DIR writes what the last timed step computed (final state, times, last step sizes and the propagate
+results) as DIR/<name>.npy, float64, for a fixed seeded sample of lanes (DIR/lanes.npy), so that two builds can be
+compared output for output. Nothing is written inside the repository: what has to be compiled at run time goes to a
+temporary directory.
 """
 import argparse
 import json
 import os
 import subprocess
 import sys
+import tempfile
 import threading
 import time
 
@@ -50,7 +56,17 @@ def parse_args():
     ap.add_argument("--lanes-per-thread", type=int, default=0)
     ap.add_argument("--block-threads", type=int, default=0)
     ap.add_argument("--blocks-per-sm", type=int, default=0)
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="write the outputs of the last timed step as DIR/<name>.npy")
     return ap.parse_args()
+
+
+# NVIDIA's data sheet for the H100 SXM (700 W): HBM3 bandwidth and the FP64 (non-tensor) rate of the DFMA pipe.
+H100_HBM_GBS = 3350.0
+H100_FP64_TFLOPS = 34.0
+
+# Upper bound on the bytes --dump-outputs writes.
+DUMP_MAX_BYTES = 48 << 20
 
 
 def measured_peaks():
@@ -58,30 +74,26 @@ def measured_peaks():
     if os.path.exists(path):
         with open(path) as f:
             return json.load(f), "measured"
-    return {"hbm_gbs": 6650.0}, "fallback"
+    return {"hbm_gbs": H100_HBM_GBS}, "data sheet (H100 SXM)"
 
 
-def measured_traffic(kernel_kind, lane_steps_per_launch):
-    """DRAM bytes per launch of the dominant kernel from this round's committed `ncu --set full` capture
-    (profiles/r2_traffic.json, written by profiles/summarise_ncu.py: dram__bytes_read.sum + dram__bytes_write.sum, the
-    lane-steps of the profiled launch and the FP64 pipe utilisation); the kernel's DRAM traffic is proportional to the
-    lane-steps. Returns (bytes per launch, capture record) or (None, None)."""
-    path = os.path.join(ROOT, "profiles", "r2_traffic.json")
-    try:
-        with open(path) as f:
-            t = json.load(f)[kernel_kind]
-        return float(t["dram_bytes"]) / float(t["lane_steps"]) * lane_steps_per_launch, t
-    except (OSError, KeyError, ValueError):
-        return None, None
-
-
-def measured_fp64_peak():
-    """FP64 peak of the chip, measured by tools/fp64_peak.cu (dependency-free DFMA streams), profiles/r2_fp64_peak.json."""
-    try:
-        with open(os.path.join(ROOT, "profiles", "r2_fp64_peak.json")) as f:
-            return float(json.load(f)["dfma_tflops"]), "measured (tools/fp64_peak.cu)"
-    except (OSError, KeyError, ValueError):
-        return 37.0, "fallback"
+def dump_outputs(out_dir, n_eq, n, arrays):
+    """Writes a fixed, seeded sample of lanes of the final state [n_eq, n] and of the per-lane arrays as float64 .npy
+    files (at most DUMP_MAX_BYTES in all). `arrays`: name -> device tensor; "state" is [n_eq * n], the others [n]."""
+    import torch
+    per_lane = (n_eq + len(arrays)) * 8  # state rows + the other arrays (one replaced by lanes.npy)
+    k = min(n, (DUMP_MAX_BYTES - 4096) // per_lane)
+    lanes = np.arange(n) if k == n else np.sort(np.random.default_rng(20240601).choice(n, size=k, replace=False))
+    os.makedirs(out_dir, exist_ok=True)
+    np.save(os.path.join(out_dir, "lanes.npy"), lanes.astype(np.float64))
+    for name, t in arrays.items():
+        dev = t.device
+        idx = torch.from_numpy(lanes).to(dev)
+        if name == "state":
+            v = t.view(n_eq, n).index_select(1, idx)
+        else:
+            v = t.index_select(0, idx)
+        np.save(os.path.join(out_dir, name + ".npy"), v.to(torch.float64).cpu().numpy())
 
 
 class ClockSampler:
@@ -166,6 +178,9 @@ class CpuBaseline:
         import oracle
         from common import outer_ss_batch_state
         self.P, self.cores, self.oracle, self.codegen = P, cores, oracle, codegen
+        # The generated code is compiled outside of the source tree (which may be read-only).
+        self._build_dir = tempfile.TemporaryDirectory(prefix="heyoka_codegen_")
+        codegen.BUILD = self._build_dir.name
         self.jets = {w: codegen.Jet(P, w) for w in (4, 8)}  # compiled outside of every timed region
         cal = outer_ss_batch_state(8 * cores, perturb=perturb, seed=7)
         self.rates = {}
@@ -255,17 +270,15 @@ def run_reference(args):
 def cpp_class_e2e(batch, tfinal, perturb):
     """The same workload through the drop-in C++ class (tools/bench_cpp_e2e.cpp): host std::vector buffers in and out,
     the call a heyoka user makes. One line per host_sync mode; None if the tool cannot be built."""
-    exe = os.path.join(ROOT, "build", "bench_cpp_e2e")
     src = os.path.join(ROOT, "tools", "bench_cpp_e2e.cpp")
     lib = os.path.join(ROOT, "heyoka_b200", "lib")
     try:
-        if not os.path.exists(exe) or os.path.getmtime(exe) < max(os.path.getmtime(src), os.path.getmtime(
-                os.path.join(lib, "libheyoka_b200.so"))):
-            os.makedirs(os.path.dirname(exe), exist_ok=True)
+        with tempfile.TemporaryDirectory(prefix="heyoka_bench_") as tmp:
+            exe = os.path.join(tmp, "bench_cpp_e2e")
             subprocess.run(["g++", "-std=c++17", "-O2", "-I" + os.path.join(ROOT, "include"), src, "-o", exe, "-L" + lib,
-                            "-lheyoka_b200", "-Wl,-rpath," + lib], check=True, capture_output=True)
-        res = subprocess.run([exe, str(batch), "2", repr(float(tfinal)), repr(float(perturb))], capture_output=True,
-                             text=True, timeout=600, check=True)
+                                "-lheyoka_b200", "-Wl,-rpath," + lib], check=True, capture_output=True)
+            res = subprocess.run([exe, str(batch), "2", repr(float(tfinal)), repr(float(perturb))], capture_output=True,
+                                 text=True, timeout=600, check=True)
         return [json.loads(line) for line in res.stdout.splitlines() if line.startswith("{")]
     except Exception as e:  # noqa: BLE001 - a reported extra, never fatal for the bench line
         return {"error": "%s: %s" % (type(e).__name__, e)}
@@ -381,6 +394,11 @@ def main():
         assert bool(torch.equal(g[rank, :P.n_eq * n], t_state)), "the gathered block differs from the local state"
     launches = b.launch_count() - launches0
     clocks = sampler.stop() if rank == 0 else None
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, P.n_eq, n, {
+            "state": t_state, "t_hi": t_thi, "t_lo": t_tlo, "last_h": small[2], "prop_min_h": small[3],
+            "prop_max_h": small[4], "prop_outcome": as_tensor(ptrs.prop_outcome, n, torch.int64),
+            "prop_n_steps": t_nsteps})
 
     # ---- end-to-end through the host-buffer API: pinned host -> device, propagate, device -> pinned host ----
     h_state = torch.from_numpy(st_host).pin_memory()
@@ -444,8 +462,7 @@ def main():
         # roofline of the dominant kernel (k_propagate) on this rank: algorithmic bytes / launch duration
         ach = lane_steps_rank * costs["b_tape"] / (k_ms * 1e-3) / 1e9
         peak = float(peaks["hbm_gbs"])
-        traffic, capture = measured_traffic(kinfo["tape"], lane_steps_rank)
-        fp64_peak, fp64_peak_kind = measured_fp64_peak()
+        fp64_peak, fp64_peak_kind = H100_FP64_TFLOPS, "data sheet (H100 SXM, FP64 non-tensor)"
         fp64_model = lane_steps_rank * costs["flops"] / (k_ms * 1e-3) / 1e12
         out = {
             "metric": "taylor_lane_steps_per_s", "value": value, "unit": "lane-steps/s", "n_gpus": world,
@@ -456,23 +473,17 @@ def main():
                             "propagate_until(%g yr) per step" % (P.order, n, args.tfinal),
                 "n_eq": P.n_eq, "n_uvars": P.n_uvars, "order": P.order, "lanes_per_gpu": n,
                 "lane_steps_per_step": lane_steps_all, "perturb": args.perturb,
-                "cache": "inputs larger than L2: state %.0f MB + per-warp derivative tapes (GBs) vs 126 MB of L2; ICs "
+                "cache": "inputs larger than L2: state %.0f MB + per-warp derivative tapes (GBs) vs 50 MB of L2; ICs "
                          "restored device-to-device before every step" % (state_bytes / 1e6),
                 "parallelism": "lanes sharded across %d GPU(s), final-state all_gather" % world,
             },
             "roofline": {"bound": "hbm", "achieved": ach, "peak": peak, "unit": "GB/s", "frac": ach / peak,
-                         "traffic": traffic, "peak_kind": peak_kind,
-                         # What really bounds the kernel: it moves ~20 B of DRAM traffic per lane-step (the tape lives
-                         # on chip), so the contract's B_tape figure above is an algorithmic equivalent; the binding
-                         # resources are the FP64 pipe and instruction issue.
+                         "peak_kind": peak_kind,
+                         # What really bounds the kernel: the tape lives on chip, so the B_tape figure above is an
+                         # algorithmic equivalent; the binding resources are the FP64 pipe and instruction issue.
                          "true_bound": "fp64 pipe / instruction issue",
                          "fp64_peak_tflops": fp64_peak, "fp64_peak_kind": fp64_peak_kind,
                          "fp64_frac": fp64_model / fp64_peak,
-                         "fp64_pipe_pct": None if capture is None else capture.get("fp64_pipe_pct"),
-                         "warp_inst_per_lane_step": None if capture is None else capture.get("warp_inst_per_lane_step"),
-                         "dram_bytes_per_lane_step": None if capture is None
-                         else capture["dram_bytes"] / capture["lane_steps"],
-                         "capture": None if capture is None else capture.get("source"),
                          "kernel": ("k_nb<LT=%d,prop>" % kinfo["lanes_per_warp"]) if kinfo["tape"].startswith("nbody")
                          else ("k_coop<L=%d,N=%d,prop>" % (kinfo["lanes_per_warp"], kinfo["lanes_per_thread"])
                                if kinfo["tape"] == "smem" else "k_hbm<prop>"), "kernel_config": kinfo,

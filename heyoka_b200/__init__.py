@@ -1,9 +1,9 @@
-"""heyoka_b200 — B200-native batch Taylor integrator (drop-in for heyoka's taylor_adaptive_batch<double>).
+"""heyoka_b200 — H100-native batch Taylor integrator (drop-in for heyoka's taylor_adaptive_batch<double>).
 
 This Python package is a thin ctypes mirror of the C ABI in include/heyoka_b200.h, shaped after the
 reference's C++ API (include/heyoka/taylor.hpp:780-1121) so that the parity tests read like the
 reference's own tests (test/taylor_adaptive_batch.cpp). The product is the native library
-(heyoka_b200/lib/libheyoka_b200.so: host C++ front end + hand-written sm_100a CUDA kernels); there is no
+(heyoka_b200/lib/libheyoka_b200.so: host C++ front end + hand-written sm_90a CUDA kernels); there is no
 Python or CPU fallback for the compute path: if the library is missing, importing fails loudly.
 """
 import ctypes as C
@@ -334,8 +334,8 @@ class Batch:
         check(lib.hy_batch_set_launch_config(self._h, int(block_threads), int(blocks_per_sm)))
 
     def set_kernel(self, tape="auto", lanes_per_warp=0, lanes_per_thread=0, block_threads=0, blocks_per_sm=0):
-        # "nbody" / "nbody-cta": the dedicated N-body kernel (warp / CTA teams); lanes_per_thread then selects the
-        # storage of the private rows: 0 automatic, 1 tensor memory, 2 shared memory only.
+        # "nbody" / "nbody-cta": the dedicated N-body kernel (warp / CTA teams; lanes_per_thread is ignored).
+        # "smem-notmem" is the same as "smem" (kept for compatibility).
         # "nn": the dense-network kernel (right-hand sides that are feed-forward networks).
         mode = {"auto": 0, "hbm": 1, "smem": 2, "smem-notmem": 3, "global": 4, "global-cta": 5, "nbody": 6,
                 "nbody-cta": 7, "nn": 8, "nbody-lane": 9}[tape]

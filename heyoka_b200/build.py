@@ -1,10 +1,9 @@
-"""Build the native library (host C++ + sm_100a CUDA) in-tree with nvcc.
+"""Build the native library (host C++ + sm_90a CUDA) in-tree with nvcc.
 
     python -m heyoka_b200.build [--force]
 
-Output: heyoka_b200/lib/libheyoka_b200.so (git-ignored, travels to the GPU box with the snapshot).
-nvcc cross-compiles for sm_100a without a GPU. -fmad=false: the only fused multiply-adds are the
-explicit fma() calls in csrc/recurrences.cuh (see the floating-point contract there).
+Output: heyoka_b200/lib/libheyoka_b200.so (git-ignored). nvcc cross-compiles for sm_90a (H100) without a GPU.
+-fmad=false: the only fused multiply-adds are the explicit fma() calls in csrc/recurrences.cuh (see the floating-point contract there).
 """
 import os
 import shutil
@@ -24,13 +23,12 @@ CUDA_SOURCES = ["batch.cu", "nn_inst.cu", "nb1_inst.cu"]
 # The cooperative kernel is instantiated per (lanes per thread, max threads per CTA, mode) family, one
 # object each (built in parallel).
 COOP_FAMILIES = ([(n, m, g) for n in (1, 2, 4) for m in (512, 256) for g in (1, 0)]
-                 + [(n, m, g) for n in (1, 2) for m in (512, 384, 256) for g in (2, 3)]
                  + [(1, 512, 4), (2, 512, 4), (1, 512, 5), (2, 512, 5)])
 
 # The dedicated N-body kernel: one object per (lanes per team, CTA-wide team) family.
 NB_FAMILIES = [(lt, 0) for lt in (1, 2, 4, 8, 16, 32)] + [(1, 1)]
 
-NVCC_ARCH = ["-gencode", "arch=compute_100a,code=sm_100a"]
+NVCC_ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 CUDA_FLAGS = ["-lineinfo", "-fmad=false", "-Xcompiler", "-fPIC", "-Xptxas", "-v"]
 COMMON = ["-std=c++17", "-O3", "-I" + os.path.join(ROOT, "include"), "-I" + CSRC]
 
@@ -64,7 +62,7 @@ def build(force=False, verbose=True):
     hdrs = _all_headers()
     srcs = [os.path.join(CSRC, f) for f in HOST_SOURCES + CUDA_SOURCES + ["coop_inst.cu", "nb_inst.cu"]]
     if not force and not _deps_newer(LIB, srcs + hdrs):
-        return LIB  # up to date (the objects under build/ do not travel to the GPU box)
+        return LIB  # up to date
     jobs = []  # (obj, deps, cmd)
     for src in HOST_SOURCES + CUDA_SOURCES:
         path = os.path.join(CSRC, src)

@@ -55,7 +55,7 @@ namespace
 using hy::detail::coop_variant;
 
 // maxt: upper bound on the threads per CTA the variant was compiled for (256: up to 255 registers per thread).
-// mode: 1 = the plan contains elementary ops, 0 = superinstructions only, 2 / 3 = idem with tensor memory,
+// mode: 1 = the plan contains elementary ops, 0 = superinstructions only,
 // 4 = any plan, tape and tables in global memory, 5 = idem with the whole CTA working on one chunk of lanes.
 const coop_variant *find_variant(int L, int N, int maxt, int mode)
 {
@@ -72,18 +72,6 @@ const coop_variant *find_variant(int L, int N, int maxt, int mode)
         hy::detail::coop_family_n4_512_m0(),
         hy::detail::coop_family_n4_256_m1(),
         hy::detail::coop_family_n4_256_m0(),
-        hy::detail::coop_family_n1_512_m2(),
-        hy::detail::coop_family_n1_512_m3(),
-        hy::detail::coop_family_n1_384_m2(),
-        hy::detail::coop_family_n1_384_m3(),
-        hy::detail::coop_family_n1_256_m2(),
-        hy::detail::coop_family_n1_256_m3(),
-        hy::detail::coop_family_n2_512_m2(),
-        hy::detail::coop_family_n2_512_m3(),
-        hy::detail::coop_family_n2_384_m2(),
-        hy::detail::coop_family_n2_384_m3(),
-        hy::detail::coop_family_n2_256_m2(),
-        hy::detail::coop_family_n2_256_m3(),
         hy::detail::coop_family_n1_512_m4(),
         hy::detail::coop_family_n2_512_m4(),
         hy::detail::coop_family_n1_512_m5(),
@@ -99,7 +87,7 @@ const coop_variant *find_variant(int L, int N, int maxt, int mode)
 }
 
 // The N-body kernel's instantiations (nb_variants.hpp).
-const hy::detail::nb_variant *find_nb_variant(int LT, bool cta, bool tmem, int maxt, bool lane = false)
+const hy::detail::nb_variant *find_nb_variant(int LT, bool cta, bool offchip, int maxt, bool lane = false)
 {
     const hy::detail::nb_family fams[] = {hy::detail::nb_family_lt1_cta0(),  hy::detail::nb_family_lt2_cta0(),
                                           hy::detail::nb_family_lt4_cta0(),  hy::detail::nb_family_lt8_cta0(),
@@ -107,7 +95,7 @@ const hy::detail::nb_variant *find_nb_variant(int LT, bool cta, bool tmem, int m
                                           hy::detail::nb_family_lt1_cta1(),  hy::detail::nb_family_lane()};
     for (const auto &f : fams) {
         for (std::size_t i = 0; i < f.n; ++i) {
-            if (f.v[i].LT == LT && f.v[i].cta == cta && f.v[i].tmem == tmem && f.v[i].maxt == maxt
+            if (f.v[i].LT == LT && f.v[i].cta == cta && f.v[i].offchip == offchip && f.v[i].maxt == maxt
                 && f.v[i].lane == lane) {
                 return f.v + i;
             }
@@ -134,7 +122,6 @@ std::vector<std::uint32_t> make_plan_blob(const hy::detail::smem_plan &pl, const
     h.n_eq = p.n_eq;
     h.n_slots = pl.n_slots;
     h.n_gslots = pl.n_gslots;
-    h.tmem = pl.tmem;
     align(4);
     h.off_ops = static_cast<std::uint32_t>(b.size());
     for (std::size_t i = 0; i < pl.ops.size(); ++i) {
@@ -220,9 +207,7 @@ struct hy_batch {
     std::shared_ptr<const hy_program> prog_host; // kept for re-planning
     bool opt_fuse = true, opt_fuse_sv = true;
     int opt_spill = -1; // -1 automatic, 0 never, 1 always
-    bool opt_tmem = true, allow_tmem = true;
-    std::uint32_t opt_tmem_rows = 0; // 0: automatic, 2 / 3: forced (HEYOKA_B200_TMEM_ROWS)
-    void replan(bool spill, std::uint32_t tmem_max_pairs = 0, std::uint32_t tmem_rows = 2);
+    void replan(bool spill);
     void ensure_tc();
     void setup_coop_global(int L, int N, std::uint32_t threads, int cta = -1);
     bool c_cta = false; // ... and the whole CTA working on one chunk of lanes (kernel mode 5)
@@ -238,7 +223,7 @@ struct hy_batch {
     coop_variant nb_cv{}; // (L, N, maxt, mode 6) of the selected N-body instantiation, for the code that reads cv->L
     bool nb_on = false;
     int opt_nb = -1; // -1 automatic, 0 never (HEYOKA_B200_NB=0), 1 preferred
-    bool setup_nb(int LT, std::uint32_t threads, int want_tmem, int want_cta, int want_lane = 0);
+    bool setup_nb(int LT, std::uint32_t threads, int want_cta, int want_lane = 0);
     int opt_nb_lane = -1; // one thread per lane for single-pair systems: -1 automatic, 0 never (HEYOKA_B200_NB_LANE=0)
     bool nb_lane = false;
     // The dense-network kernel (nn_kernel.cuh): plan, padded weight image, device plan.
@@ -423,9 +408,9 @@ void hy_batch::setup_hbm(std::uint32_t threads, std::uint32_t blocks_per_sm)
     mode = 1;
 }
 
-void hy_batch::replan(bool spill, std::uint32_t tmem_max_pairs, std::uint32_t tmem_rows)
+void hy_batch::replan(bool spill)
 {
-    plan = hy::detail::make_smem_plan(*prog_host, opt_fuse, opt_fuse_sv, spill, tmem_max_pairs, tmem_rows);
+    plan = hy::detail::make_smem_plan(*prog_host, opt_fuse, opt_fuse_sv, spill);
     const auto blob = make_plan_blob(plan, *prog_host);
     if (d_blob != nullptr) {
         HY_CUDA_CHECK(cudaFree(d_blob));
@@ -440,7 +425,6 @@ void hy_batch::replan(bool spill, std::uint32_t tmem_max_pairs, std::uint32_t tm
 bool hy_batch::setup_coop(int L, int N, std::uint32_t threads, std::uint32_t ctas_per_sm)
 {
     const std::size_t reserve = 1024u; // per-block reservation of the driver
-    const bool auto_shape = N == 0 && L == 0;
     if (N == 0) {
         // Two lanes per thread: the interpreter's per-item overhead is shared and the recurrences get ILP 2.
         N = (L == 0 || L >= 2) ? 2 : 1;
@@ -452,8 +436,8 @@ bool hy_batch::setup_coop(int L, int N, std::uint32_t threads, std::uint32_t cta
     {
         const bool have_spill = plan.n_gslots != 0u;
         const bool want_spill = opt_spill > 0;
-        if (want_spill != have_spill || plan.tmem) {
-            replan(want_spill); // (the tensor-memory decision is taken again below for this L, N)
+        if (want_spill != have_spill) {
+            replan(want_spill);
         }
     }
     if (L == 0) {
@@ -489,95 +473,27 @@ bool hy_batch::setup_coop(int L, int N, std::uint32_t threads, std::uint32_t cta
         }
         return std::min<std::size_t>((smem_per_block_max - reserve - blob_bytes) / wb, 16u);
     };
-    // Tensor memory (HEYOKA_B200_TMEM=0 disables): if the program consists of superinstructions only, with at
-    // most one pair interaction per thread of a warp, the history rows that only their own thread touches (r^2,
-    // r^alpha, optionally one of the coordinate differences) can live in TMEM (one TMEM lane per thread, 512
-    // columns shared by the warps of a quadrant) instead of shared memory. Taken when it lets more warps reside
-    // on an SM. 6-body system, order 20: 8 warps of 2 lanes without TMEM; 12 with two rows of 2 lanes per thread
-    // in TMEM; 16 with three rows of 1 lane per thread (2 lanes per warp, 30 busy threads in the pair level).
-    const auto tm_warps_of = [&](int lanes_per_thread, std::uint32_t rows) -> std::size_t {
-        const std::uint32_t cols = rows * (order + 1u) * 2u * static_cast<std::uint32_t>(lanes_per_thread);
-        return cols <= 512u ? 4u * (512u / cols) : 0u;
-    };
-    struct tm_choice {
-        std::uint32_t rows = 0;
-        std::size_t warps = 0;
-    };
-    const auto best_tmem = [&](int lanes, int lanes_per_thread) {
-        tm_choice best;
-        const std::uint32_t G = static_cast<std::uint32_t>(lanes / lanes_per_thread);
-        if (!(opt_tmem && allow_tmem && lanes_per_thread <= 2 && G != 0u && G <= 32u && opt_spill <= 0)) {
-            return best;
-        }
-        for (const std::uint32_t rows : {2u, 3u}) {
-            if ((opt_tmem_rows != 0u && rows != opt_tmem_rows)
-                || find_variant(lanes, lanes_per_thread, 512, static_cast<int>(rows)) == nullptr) {
-                continue;
-            }
-            const auto cand = hy::detail::make_smem_plan(*prog_host, opt_fuse, opt_fuse_sv, false, 32u / G, rows);
-            if (cand.tmem != rows) {
-                continue;
-            }
-            const auto w = std::min(fit_warps(cand.n_slots, lanes), tm_warps_of(lanes_per_thread, rows));
-            if (w > best.warps) {
-                best = tm_choice{rows, w};
-            }
-        }
-        return best;
-    };
-    {
-        tm_choice pick = best_tmem(L, N);
-        if (auto_shape && plan.n_fused != 0u && plan.n_fused <= 32u) {
-            // The tensor-memory shape of choice: 1 lane per thread and as many lanes per warp as give every thread
-            // one pair interaction (15 pairs: 2 lanes, 30 busy threads; 1 pair: 32 lanes). Taken when it puts
-            // more lanes in flight on an SM.
-            int alt_l = 1;
-            while (static_cast<std::uint32_t>(2 * alt_l) * plan.n_fused <= 32u) {
-                alt_l *= 2;
-            }
-            const auto alt = best_tmem(alt_l, 1);
-            if (alt.warps * static_cast<std::size_t>(alt_l)
-                > std::max(pick.warps, fit_warps(plan.n_slots, L)) * static_cast<std::size_t>(L)) {
-                pick = alt;
-                L = alt_l;
-                N = 1;
-            }
-        }
-        if (pick.rows != 0u && pick.warps > fit_warps(plan.n_slots, L)) {
-            replan(false, 32u / static_cast<std::uint32_t>(L / N), pick.rows);
-            // Level 0 must be exactly the pair interactions, at most one per thread.
-            const auto b0 = plan.seg_offsets[0], e0 = plan.seg_offsets[1];
-            bool ok = plan.tmem == pick.rows && (e0 - b0) * static_cast<std::uint32_t>(L / N) <= 32u;
-            for (std::size_t i = 0; i < plan.ops.size(); ++i) {
-                ok = ok && ((plan.ops[i].opcode == hy::detail::HY_FOP_NBODY_PAIR) == (i >= b0 && i < e0));
-            }
-            if (!ok) {
-                throw std::logic_error("Inconsistent tensor-memory plan");
-            }
-        }
-    }
     const auto warp_bytes = coop_warp_bytes(plan.n_slots, L);
     if (blob_bytes > 24u * 1024u || blob_bytes + warp_bytes + reserve > smem_per_block_max) {
         return false;
     }
-    const std::size_t tm_warp_limit = plan.tmem != 0u ? tm_warps_of(N, plan.tmem) : 16u;
     if (threads == 0u) {
-        // One CTA per SM holding as many warps as fit (shared memory, tensor-memory columns).
-        const std::size_t W = std::min(fit_warps(plan.n_slots, L), tm_warp_limit);
+        // One CTA per SM holding as many warps as fit in shared memory.
+        const std::size_t W = fit_warps(plan.n_slots, L);
         threads = static_cast<std::uint32_t>(32u * std::max<std::size_t>(W, 1u));
     }
-    if (threads % 32u != 0u || threads == 0u || threads > 512u || threads / 32u > tm_warp_limit) {
+    if (threads % 32u != 0u || threads == 0u || threads > 512u) {
         throw std::invalid_argument("Invalid number of threads for the cooperative kernel");
     }
     // Registers: 65536 / 512 threads = 128 per thread, 170 with at most 384 threads, 255 with at most 256.
-    int kmode = static_cast<int>(plan.tmem); // 0, 2 or 3
+    int kmode = 0;
     for (const auto &op : plan.ops) {
         kmode = op.opcode < hy::detail::HY_FOP_FIRST ? 1 : kmode;
     }
     // (Not every shape is compiled for every CTA size: fall back to the next larger bound.)
-    const int pref_maxt = threads <= 256u ? 256 : (threads <= 384u && kmode >= 2 ? 384 : 512);
+    const int pref_maxt = threads <= 256u ? 256 : 512;
     const coop_variant *v = nullptr;
-    for (const int m : {256, 384, 512}) {
+    for (const int m : {256, 512}) {
         if (m >= pref_maxt && v == nullptr) {
             v = find_variant(L, N, m, kmode);
         }
@@ -629,7 +545,7 @@ bool hy_batch::setup_coop(int L, int N, std::uint32_t threads, std::uint32_t cta
 // thousand lanes (a warp works on L lanes, its threads on different u variables).
 void hy_batch::setup_coop_global(int L, int N, std::uint32_t threads, int cta)
 {
-    if (plan.tmem != 0u || plan.n_gslots != 0u) {
+    if (plan.n_gslots != 0u) {
         replan(false);
     }
     if (N == 0) {
@@ -755,9 +671,9 @@ static bool make_nb1_tab(const hy::detail::nb_plan &pl, std::uint32_t n_eq, std:
 }
 
 // The dedicated N-body kernel. LT = lanes per team (0: as many as give every thread of a warp one pair interaction),
-// threads = CTA size (0: as many warps as fit; HEYOKA_B200_NB_THREADS caps it), want_tmem / want_cta: -1 automatic.
+// threads = CTA size (0: as many warps as fit; HEYOKA_B200_NB_THREADS caps it), want_cta: -1 automatic.
 // Returns false if the program does not qualify or nothing fits.
-bool hy_batch::setup_nb(int LT, std::uint32_t threads, int want_tmem, int want_cta, int want_lane)
+bool hy_batch::setup_nb(int LT, std::uint32_t threads, int want_cta, int want_lane)
 {
     if (!nbp.ok) {
         return false;
@@ -809,35 +725,31 @@ bool hy_batch::setup_nb(int LT, std::uint32_t threads, int want_tmem, int want_c
         }
         return d;
     };
-    const auto team_slots = [&](bool tmem) {
+    const auto team_slots = [&](bool offchip) {
         // (The one-thread-per-lane kernel keeps positions, pair outputs and norms in registers.)
         const std::size_t d = (lane ? 0u : (static_cast<std::size_t>(nbp.n_pos) + nbp.n_out) * LT * 2u)
-                              + static_cast<std::size_t>(tmem ? 2u : 5u) * npp * TT * 2u
+                              + static_cast<std::size_t>(offchip ? 2u : 5u) * npp * TT * 2u
                               + (3u * hy::detail::nb_norm_copies(static_cast<std::uint32_t>(LT)) + 16u) * LT; // (+ norms, parked bookkeeping)
         return static_cast<std::uint32_t>((d + LT - 1u) / LT);
     };
-    // Teams (warps) per CTA that fit: shared memory, tensor-memory columns (12 per order pair and thread).
+    // Teams (warps) per CTA that fit in shared memory. CTA teams whose five private rows per thread do not fit keep
+    // three of them (r^2, d_2, r^alpha) off chip, in a per-CTA slab of global memory that stays in L2.
     struct choice {
-        bool tmem = false, roles_in_smem = false;
+        bool offchip = false, roles_in_smem = false;
         std::uint32_t warps = 0;
     };
-    const auto fit = [&](bool tmem) {
+    const auto fit = [&](bool offchip) {
         choice c;
-        c.tmem = tmem;
+        c.offchip = offchip;
         for (const bool ris : {true, false}) {
             const std::size_t sh = shared_doubles(ris) * sizeof(double);
-            const std::size_t tb = coop_warp_bytes(team_slots(tmem), LT);
+            const std::size_t tb = coop_warp_bytes(team_slots(offchip), LT);
             if (sh + tb + reserve > smem_per_block_max) {
                 continue;
             }
             std::uint32_t w = cta ? 16u
                                   : static_cast<std::uint32_t>(
                                         std::min<std::size_t>((smem_per_block_max - reserve - sh) / tb, 16u));
-            if (tmem) {
-                const std::uint32_t cols = npp * 12u;
-                const std::uint32_t per_quadrant = cols == 0u || cols > 512u ? 0u : 512u / cols;
-                w = std::min(w, 4u * per_quadrant);
-            }
             if (cta && w < 16u) {
                 w = 0u;
             }
@@ -851,15 +763,9 @@ bool hy_batch::setup_nb(int LT, std::uint32_t threads, int want_tmem, int want_c
         }
         return c;
     };
-    choice pick;
-    if (want_tmem != 0 && opt_tmem) {
+    choice pick = fit(false);
+    if (cta && pick.warps == 0u) {
         pick = fit(true);
-    }
-    if (want_tmem <= 0) {
-        const auto alt = fit(false);
-        if (alt.warps > pick.warps) {
-            pick = alt;
-        }
     }
     if (pick.warps == 0u) {
         return false;
@@ -882,7 +788,7 @@ bool hy_batch::setup_nb(int LT, std::uint32_t threads, int want_tmem, int want_c
     const hy::detail::nb_variant *v = nullptr;
     for (const int mt : {256, 384, 512}) {
         if (mt >= pref_maxt && v == nullptr) {
-            v = find_nb_variant(LT, cta, pick.tmem, mt, lane);
+            v = find_nb_variant(LT, cta, pick.offchip, mt, lane);
         }
     }
     if (v == nullptr) {
@@ -916,7 +822,7 @@ bool hy_batch::setup_nb(int LT, std::uint32_t threads, int want_tmem, int want_c
     nbd.pow_algo = nbp.pow_algo;
     nbd.roles_in_smem = pick.roles_in_smem ? 1u : 0u;
     nbd.shared_doubles = static_cast<std::uint32_t>(shared_doubles(pick.roles_in_smem));
-    nbd.n_slots_equiv = team_slots(pick.tmem);
+    nbd.n_slots_equiv = team_slots(pick.offchip);
     nbd.l1 = l1;
     nb_lane = lane;
     const std::size_t team_bytes = coop_warp_bytes(nbd.n_slots_equiv, LT);
@@ -943,6 +849,10 @@ bool hy_batch::setup_nb(int LT, std::uint32_t threads, int want_tmem, int want_c
     c_grid = std::max(1u, std::min(n_sms, n_blocks_needed));
     d_cscratch = dalloc<double>(static_cast<std::size_t>(c_grid) * teams * (order + 1u) * n_eq
                                 * static_cast<std::size_t>(LT));
+    if (pick.offchip) {
+        d_gscratch = dalloc<double>(static_cast<std::size_t>(c_grid) * npp * 3u * TT * 2u);
+        nbd.offchip = d_gscratch;
+    }
     mode = 2;
     nb_on = true;
     c_cta = cta;
@@ -959,7 +869,7 @@ bool hy_batch::setup_nn()
     }
     dev::nn_dev_plan d{};
     std::vector<double> img;
-    std::uint32_t hist = 0, max_out = 0, n_hidden = 0;
+    std::uint32_t hist = 0, max_out = 0;
     d.n_layers = static_cast<std::uint32_t>(nnp.layers.size());
     for (std::uint32_t l = 0; l < d.n_layers; ++l) {
         const auto &L = nnp.layers[l];
@@ -985,16 +895,9 @@ bool hy_batch::setup_nn()
         img.resize((img.size() + 1u) & ~std::size_t(1), 0.);
         d.hist_off[l] = hist;
         if (L.act != 0) {
-            hist += 2u * order * L.n_out * dev::NN_LB; // z and the activation (its square lives in tensor memory)
-            d.tm_slot[l] = n_hidden++;
-            d.tm_ipt = std::max(d.tm_ipt, (L.n_out * dev::NN_LB + dev::NN_THREADS - 1u) / dev::NN_THREADS);
+            hist += 3u * order * L.n_out * dev::NN_LB; // z, the activation and its square
         }
         max_out = std::max(max_out, L.n_out);
-    }
-    // Tensor memory: 48 columns per (neuron, lane) item and hidden layer (16 of padding + 2 per order), 256 columns per
-    // thread, orders up to 16 (the history is read back in two windows of eight orders).
-    if (n_hidden * d.tm_ipt * 48u > 256u || order > 16u) {
-        return false;
     }
     d.wimg_doubles = static_cast<std::uint32_t>(img.size());
     d.hist_doubles = hist;
@@ -1055,14 +958,13 @@ void hy_batch::configure(int want_mode, int L, int N, std::uint32_t threads, std
                                         + (nnp.ok ? std::string("it does not fit in shared memory") : nnp.why));
         }
     }
-    // Mode 6 / 7: the N-body kernel with warp / CTA teams (N: 0 automatic, 1 tensor memory, 2 shared memory only).
+    // Mode 6 / 7: the N-body kernel with warp / CTA teams.
     // Automatic mode takes it whenever the program qualifies (nb_plan.hpp).
     if (want_mode == 6 || want_mode == 7 || want_mode == 9 || (want_mode == 0 && opt_nb != 0)) {
         // Mode 9: one thread per lane (systems with one pair interaction); the automatic mode takes it when it applies,
         // an explicit mode 6 never does (it selects k_nb with the given team shape).
         const int want_lane = want_mode == 9 ? 1 : (want_mode == 0 ? (opt_nb_lane != 0 ? -1 : 0) : 0);
-        if (setup_nb(want_mode == 9 ? 32 : L, threads, N == 0 ? -1 : (N == 1 ? 1 : 0),
-                     want_mode == 0 ? -1 : (want_mode == 7 ? 1 : 0), want_lane)) {
+        if (setup_nb(want_mode == 9 ? 32 : L, threads, want_mode == 0 ? -1 : (want_mode == 7 ? 1 : 0), want_lane)) {
             return;
         }
         if (want_mode != 0) {
@@ -1078,7 +980,6 @@ void hy_batch::configure(int want_mode, int L, int N, std::uint32_t threads, std
         setup_hbm(threads, blocks_per_sm);
         return;
     }
-    allow_tmem = want_mode != 3;
     if (want_mode == 3) {
         want_mode = 2;
     }
@@ -1159,6 +1060,8 @@ void hy_batch::ev_setup(std::uint32_t n_te_, const std::int32_t *dirs, const dou
     E.cd = keep(dalloc<double>(B * 2u * std::max(n_te, 1u)));
     E.cd_on = keep(dalloc<unsigned char>(B * std::max(n_te, 1u)));
     HY_CUDA_CHECK(cudaMemset(E.cd_on, 0, B * std::max(n_te, 1u)));
+    // (Inactive cooldowns read back as zeros, not as whatever the allocation held.)
+    HY_CUDA_CHECK(cudaMemset(E.cd, 0, sizeof(double) * B * 2u * std::max(n_te, 1u)));
     E.cand = keep(dalloc<std::uint32_t>(B * n_ev));
     E.counters = keep(dalloc<unsigned>(4));
     E.rec_cap = static_cast<std::uint32_t>(std::min<std::size_t>(std::max<std::size_t>(B * n_ev, 1024u), 1u << 26));
@@ -1597,8 +1500,7 @@ int hy_batch_create(const hy_program *p, uint32_t batch, int device, hy_batch **
 
         // Cooperative plan.
         // HEYOKA_B200_FUSE=0 disables the superinstructions, HEYOKA_B200_FUSE_SV=0 the fused state-variable
-        // propagation, HEYOKA_B200_SPILL=0/1 forces the overflow tape off/on, HEYOKA_B200_TMEM=0 keeps every
-        // row in shared memory (diagnostics / tests).
+        // propagation, HEYOKA_B200_SPILL=0/1 forces the overflow tape off/on (diagnostics / tests).
         if (const char *env = std::getenv("HEYOKA_B200_FUSE")) {
             b->opt_fuse = std::string{env} != "0";
         }
@@ -1607,12 +1509,6 @@ int hy_batch_create(const hy_program *p, uint32_t batch, int device, hy_batch **
         }
         if (const char *env = std::getenv("HEYOKA_B200_SPILL")) {
             b->opt_spill = std::string{env} != "0" ? 1 : 0;
-        }
-        if (const char *env = std::getenv("HEYOKA_B200_TMEM")) {
-            b->opt_tmem = std::string{env} != "0";
-        }
-        if (const char *env = std::getenv("HEYOKA_B200_TMEM_ROWS")) {
-            b->opt_tmem_rows = std::string{env} == "3" ? 3u : (std::string{env} == "2" ? 2u : 0u);
         }
         if (const char *env = std::getenv("HEYOKA_B200_NB")) {
             b->opt_nb = std::string{env} != "0" ? 1 : 0;
@@ -1761,7 +1657,10 @@ int hy_selftest_div(uint64_t n, uint64_t seed, uint64_t *mismatches)
         unsigned long long *d = nullptr;
         HY_CUDA_CHECK(cudaMalloc(&d, sizeof(unsigned long long)));
         HY_CUDA_CHECK(cudaMemset(d, 0, sizeof(unsigned long long)));
-        dev::k_selftest_div<<<148 * 8, 256>>>(n, seed, d);
+        int dev_id = 0, n_sms = 0;
+        HY_CUDA_CHECK(cudaGetDevice(&dev_id));
+        HY_CUDA_CHECK(cudaDeviceGetAttribute(&n_sms, cudaDevAttrMultiProcessorCount, dev_id));
+        dev::k_selftest_div<<<n_sms * 8, 256>>>(n, seed, d);
         HY_CUDA_CHECK(cudaGetLastError());
         unsigned long long h = 0;
         HY_CUDA_CHECK(cudaMemcpy(&h, d, sizeof(h), cudaMemcpyDeviceToHost));
@@ -1842,7 +1741,7 @@ int hy_batch_set_launch_config(hy_batch *b, uint32_t block_threads, uint32_t blo
         if (b->nn_on) {
             b->configure(8, 0, 0, 0, 0);
         } else if (b->nb_on) {
-            b->configure(b->nb_lane ? 9 : (b->c_cta ? 7 : 6), L, b->nbv->tmem ? 1 : 2, block_threads, blocks_per_sm);
+            b->configure(b->nb_lane ? 9 : (b->c_cta ? 7 : 6), L, 0, block_threads, blocks_per_sm);
         } else {
             b->configure(b->mode, L, N, block_threads, blocks_per_sm);
         }
@@ -1901,11 +1800,7 @@ int hy_batch_get_kernel(const hy_batch *b, hy_kernel_info *out)
     out->n_segments = b->plan.n_segments;
     out->n_fused = b->plan.n_fused;
     out->n_sms = b->n_sms;
-    out->tmem_cols_per_warp
-        = b->nb_on ? (b->nbv->tmem ? b->nbd.npp * 12u : 0u)
-                   : (b->mode == 2 && b->plan.tmem != 0u
-                          ? b->plan.tmem * (b->order + 1u) * 2u * static_cast<uint32_t>(b->cv->N)
-                          : 0u);
+    out->tmem_cols_per_warp = 0u; // (sm_90 has no tensor memory)
     out->reserved = 0u;
     return HY_OK;
 }

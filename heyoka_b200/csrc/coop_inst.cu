@@ -34,13 +34,6 @@ const coop_variant family[] = {
     HY_COOP(1), HY_COOP(2), HY_COOP(4)
 #elif HY_COOP_MODE == 4 && HY_COOP_N == 2
     HY_COOP(2), HY_COOP(4), HY_COOP(8)
-#elif HY_COOP_MODE >= 2 && HY_COOP_N == 1 && HY_COOP_MAXT == 512
-    // Tensor-memory variants: one pair interaction per thread (G = L lane groups x pairs <= 32).
-    HY_COOP(1), HY_COOP(2), HY_COOP(4), HY_COOP(8), HY_COOP(16), HY_COOP(32)
-#elif HY_COOP_MODE >= 2 && HY_COOP_N == 1
-    HY_COOP(1), HY_COOP(2), HY_COOP(4)
-#elif HY_COOP_MODE >= 2 && HY_COOP_N == 2
-    HY_COOP(2), HY_COOP(4)
 #elif HY_COOP_N == 1
     HY_COOP(1),  HY_COOP(2), HY_COOP(4), HY_COOP(8), HY_COOP(16), HY_COOP(32)
 #elif HY_COOP_N == 2

@@ -21,7 +21,7 @@ using coop_fn = void (*)(dev::program, const std::uint32_t *, dev::batch, dev::r
 
 struct coop_variant {
     int L, N, maxt; // lanes per warp, lanes per thread, maximum threads per CTA
-    int mode;       // 1: handles elementary ops, 0: superinstruction-only programs, 2 / 3: idem + two / three rows per pair interaction in tensor memory, 4: tape in global memory, 5: idem, CTA-wide teams
+    int mode;       // 1: handles elementary ops, 0: superinstruction-only programs, 4: tape in global memory, 5: idem, CTA-wide teams
     coop_fn step, prop;
 };
 
@@ -42,18 +42,6 @@ coop_family coop_family_n4_512_m1();
 coop_family coop_family_n4_512_m0();
 coop_family coop_family_n4_256_m1();
 coop_family coop_family_n4_256_m0();
-coop_family coop_family_n1_512_m2();
-coop_family coop_family_n1_512_m3();
-coop_family coop_family_n1_384_m2();
-coop_family coop_family_n1_384_m3();
-coop_family coop_family_n1_256_m2();
-coop_family coop_family_n1_256_m3();
-coop_family coop_family_n2_512_m2();
-coop_family coop_family_n2_512_m3();
-coop_family coop_family_n2_384_m2();
-coop_family coop_family_n2_384_m3();
-coop_family coop_family_n2_256_m2();
-coop_family coop_family_n2_256_m3();
 coop_family coop_family_n1_512_m4();
 coop_family coop_family_n2_512_m4();
 coop_family coop_family_n1_512_m5();

@@ -8,7 +8,6 @@
 #include <cstdint>
 
 #include "recurrences.cuh"
-#include "tmem.cuh"
 
 namespace heyoka_b200::dev
 {
@@ -192,321 +191,6 @@ __device__ __forceinline__ void fused_nbody_pair(const program &P, const Tape &t
             Row::store(const_cast<double *>(t.hrow(aux[17 + 4 * k]).hptr(0u)), nk);
             if (aux[30 + k] != 0u) {
                 sv_out(aux[30 + k], nk, n);
-            }
-        }
-    }
-}
-
-// The same superinstruction with its private histories in tensor memory (tmem.cuh): r^2 and r^alpha (TD == 0),
-// plus the third difference d_2 (TD == 1). Those rows are only ever touched by the thread that runs the item.
-// EVERY thread of the warp must call this function, converged (the TMEM accesses are warp-wide instructions):
-// `active` says whether this thread owns a real item; the other threads run along on the operands of another
-// item (reads only) and store nothing outside their own TMEM lane. The arithmetic is the one of
-// fused_nbody_pair(), operation by operation. TMEM rows: R2, then Q, then D2 (consecutive).
-template <int N, int TD, typename Tape, typename SvOut>
-__device__ __forceinline__ void fused_nbody_pair_tmem(const program &P, const Tape &t, const std::uint32_t *aux,
-                                                      std::uint32_t fkind, bool have_n, std::uint32_t n,
-                                                      const SvOut &sv_out, bool active, std::uint32_t tm_addr)
-{
-    using V = vd<N>;
-    using Row = typename Tape::row_t;
-    using TRow = tm::row<N>;
-    constexpr int S = static_cast<int>(Row::stride);
-    constexpr int C = 4; // orders per TMEM load
-    const std::uint32_t row_cols = (P.order + 1u) * TRow::W;
-    const TRow R2{tm_addr}, Q{tm_addr + row_cols}, D2{tm_addr + 2u * row_cols};
-    // Loads of C consecutive orders / of one order of a TMEM row.
-    const auto ldc = [](const TRow &r, std::uint32_t o, V(&out)[C]) {
-        tm::words<2 * N * C> w;
-        r.template issue<C>(o, w);
-        tm::wait_ld(w);
-        TRow::template unpack<C>(w, out);
-    };
-
-    // ---- d_k^[n] ----
-    const double *d0[3];
-#pragma unroll
-    for (int k = 0; k < 3; ++k) {
-        const V v = t.row(aux[3 * k]).at(n) - t.row(aux[3 * k + 1]).at(n);
-        if (TD == 1 && k == 2) {
-            d0[k] = nullptr;
-            D2.set(n, v);
-        } else {
-            d0[k] = t.hrow(aux[3 * k + 2]).hptr(0u);
-            if (active) {
-                Row::store(const_cast<double *>(d0[k]) + n * S, v);
-            }
-        }
-    }
-
-    // ---- r2^[n] ----
-    V r2n;
-    {
-        const bool odd = (n & 1u) != 0u;
-        V acc[3] = {splat<N>(0.), splat<N>(0.), splat<N>(0.)};
-        if (n > 0u) {
-            const std::uint32_t j1 = odd ? (n - 1u) / 2u : (n - 2u) / 2u;
-            const double *pa0 = d0[0] + n * S, *pa1 = d0[1] + n * S;
-            const double *pb0 = d0[0], *pb1 = d0[1];
-            if constexpr (TD == 0) {
-                const double *pa2 = d0[2] + n * S, *pb2 = d0[2];
-#pragma unroll 2
-                for (std::uint32_t j = 0; j <= j1; ++j) {
-                    acc[0] = vfma(Row::load(pa0), Row::load(pb0), acc[0]);
-                    acc[1] = vfma(Row::load(pa1), Row::load(pb1), acc[1]);
-                    acc[2] = vfma(Row::load(pa2), Row::load(pb2), acc[2]);
-                    pa0 -= S;
-                    pa1 -= S;
-                    pa2 -= S;
-                    pb0 += S;
-                    pb1 += S;
-                    pb2 += S;
-                }
-            } else {
-                std::uint32_t j = 0;
-                for (; j + C <= j1 + 1u; j += C) {
-                    V lo[C], hi[C]; // d2^[j + i] = lo[i], d2^[n - j - i] = hi[C - 1 - i]
-                    tm::words<2 * N * C> wl, wh;
-                    D2.template issue<C>(j, wl);
-                    D2.template issue<C>(n - j - (C - 1u), wh);
-                    tm::wait_ld(wl);
-                    tm::wait_ld(wh);
-                    TRow::template unpack<C>(wl, lo);
-                    TRow::template unpack<C>(wh, hi);
-#pragma unroll
-                    for (int i = 0; i < C; ++i) {
-                        acc[0] = vfma(Row::load(pa0), Row::load(pb0), acc[0]);
-                        acc[1] = vfma(Row::load(pa1), Row::load(pb1), acc[1]);
-                        acc[2] = vfma(hi[C - 1 - i], lo[i], acc[2]);
-                        pa0 -= S;
-                        pa1 -= S;
-                        pb0 += S;
-                        pb1 += S;
-                    }
-                }
-                for (; j <= j1; ++j) {
-                    tm::words<2 * N> wl, wh;
-                    D2.template issue<1>(j, wl);
-                    D2.template issue<1>(n - j, wh);
-                    tm::wait_ld(wl);
-                    tm::wait_ld(wh);
-                    V lo[1], hi[1];
-                    TRow::template unpack<1>(wl, lo);
-                    TRow::template unpack<1>(wh, hi);
-                    acc[0] = vfma(Row::load(pa0), Row::load(pb0), acc[0]);
-                    acc[1] = vfma(Row::load(pa1), Row::load(pb1), acc[1]);
-                    acc[2] = vfma(hi[0], lo[0], acc[2]);
-                    pa0 -= S;
-                    pa1 -= S;
-                    pb0 += S;
-                    pb1 += S;
-                }
-            }
-        }
-        V v[3];
-        if (odd) {
-#pragma unroll
-            for (int k = 0; k < 3; ++k) {
-                v[k] = acc[k];
-            }
-        } else {
-#pragma unroll
-            for (int k = 0; k < 3; ++k) {
-                const V ak2 = (TD == 1 && k == 2) ? D2.get(n / 2u) : Row::load(d0[k] + (n / 2u) * S);
-                const V sq = ak2 * ak2;
-                v[k] = n > 0u ? (acc[k] + acc[k]) + sq : sq;
-            }
-        }
-        const V r = (v[0] + v[1]) + v[2];
-        r2n = odd ? r + r : r;
-        R2.set(n, r2n);
-    }
-
-    // ---- q^[n] = pow(r2, alpha) and m_k^[n] = sum_j A^[n-j] B^[j], (A, B) = (d_k, f) or (f, d_k), f^[j] = c1 q^[j].
-    // When the products read f ascending ((A, B) = (d_k, f), the n-body case), the terms j < n of the three
-    // products are accumulated in the loop of the pow recurrence, which walks q^[0..n-1] in the same direction:
-    // one pass over the q history instead of two, four independent accumulation chains instead of one. Every
-    // accumulator still sees its own terms in its own order. ----
-    const double c1 = fkind == 1u ? t.cst(aux[14]) : (fkind == 2u ? -1. : 1.);
-    const bool f_first = aux[16] != 0u;
-    V q;
-    V acc[3] = {splat<N>(0.), splat<N>(0.), splat<N>(0.)};
-    if (!f_first) {
-        const double *pd0 = d0[0] + n * S, *pd1 = d0[1] + n * S, *pd2 = TD == 0 ? d0[2] + n * S : nullptr;
-        if (n == 0u) {
-            q = pow_eval(aux[12], r2n, splat<N>(t.cst(aux[11])));
-        } else {
-            const double nd = static_cast<double>(n);
-            const double n_alpha = nd * t.cst(aux[11]);
-            const double *jap1 = t.consts + aux[13];
-            tm::words<2 * N> w0;
-            R2.template issue<1>(0u, w0); // r2^[0] for the final division
-            V accq = splat<N>(0.);
-            std::uint32_t j = 0;
-            for (; j + C <= n; j += C) {
-                tm::words<2 * N * C> wq, wr, wd;
-                Q.template issue<C>(j, wq);
-                R2.template issue<C>(n - j - (C - 1u), wr); // r2^[n - j - i] = rv[C - 1 - i]
-                if constexpr (TD == 1) {
-                    D2.template issue<C>(n - j - (C - 1u), wd); // d2^[n - j - i] = dv[C - 1 - i]
-                }
-                tm::wait_ld(wq);
-                tm::wait_ld(wr);
-                V qv[C], rv[C], dv[C];
-                TRow::template unpack<C>(wq, qv);
-                TRow::template unpack<C>(wr, rv);
-                if constexpr (TD == 1) {
-                    tm::wait_ld(wd);
-                    TRow::template unpack<C>(wd, dv);
-                }
-#pragma unroll
-                for (int i = 0; i < C; ++i) {
-                    const double fac = n_alpha - jap1[j + i];
-                    accq = vfma(splat<N>(fac), rv[C - 1 - i] * qv[i], accq);
-                    const V fj = c1 * qv[i];
-                    acc[0] = vfma(Row::load(pd0), fj, acc[0]);
-                    acc[1] = vfma(Row::load(pd1), fj, acc[1]);
-                    acc[2] = vfma(TD == 1 ? dv[C - 1 - i] : Row::load(pd2), fj, acc[2]);
-                    pd0 -= S;
-                    pd1 -= S;
-                    if (TD == 0) {
-                        pd2 -= S;
-                    }
-                }
-            }
-            for (; j < n; ++j) {
-                tm::words<2 * N> wq, wr, wd;
-                Q.template issue<1>(j, wq);
-                R2.template issue<1>(n - j, wr);
-                if constexpr (TD == 1) {
-                    D2.template issue<1>(n - j, wd);
-                }
-                tm::wait_ld(wq);
-                tm::wait_ld(wr);
-                V qv[1], rv[1], dv[1];
-                TRow::template unpack<1>(wq, qv);
-                TRow::template unpack<1>(wr, rv);
-                if constexpr (TD == 1) {
-                    tm::wait_ld(wd);
-                    TRow::template unpack<1>(wd, dv);
-                }
-                const double fac = n_alpha - jap1[j];
-                accq = vfma(splat<N>(fac), rv[0] * qv[0], accq);
-                const V fj = c1 * qv[0];
-                acc[0] = vfma(Row::load(pd0), fj, acc[0]);
-                acc[1] = vfma(Row::load(pd1), fj, acc[1]);
-                acc[2] = vfma(TD == 1 ? dv[0] : Row::load(pd2), fj, acc[2]);
-                pd0 -= S;
-                pd1 -= S;
-                if (TD == 0) {
-                    pd2 -= S;
-                }
-            }
-            tm::wait_ld(w0);
-            V r20[1];
-            TRow::template unpack<1>(w0, r20);
-            q = accq / (nd * r20[0]);
-        }
-        Q.set(n, q);
-        // The last term of the products, j = n: d_k^[0] f^[n].
-        {
-            const V fj = c1 * q;
-            acc[0] = vfma(Row::load(pd0), fj, acc[0]);
-            acc[1] = vfma(Row::load(pd1), fj, acc[1]);
-            acc[2] = vfma(TD == 1 ? D2.get(0u) : Row::load(pd2), fj, acc[2]);
-        }
-    } else {
-        if (n == 0u) {
-            q = pow_eval(aux[12], r2n, splat<N>(t.cst(aux[11])));
-        } else {
-            const double nd = static_cast<double>(n);
-            const double n_alpha = nd * t.cst(aux[11]);
-            const double *jap1 = t.consts + aux[13];
-            tm::words<2 * N> w0;
-            R2.template issue<1>(0u, w0); // r2^[0] for the final division
-            V acc = splat<N>(0.);
-            std::uint32_t j = 0;
-            for (; j + C <= n; j += C) {
-                tm::words<2 * N * C> wq, wr;
-                Q.template issue<C>(j, wq);
-                R2.template issue<C>(n - j - (C - 1u), wr); // r2^[n - j - i] = rv[C - 1 - i]
-                tm::wait_ld(wq);
-                tm::wait_ld(wr);
-                V qv[C], rv[C];
-                TRow::template unpack<C>(wq, qv);
-                TRow::template unpack<C>(wr, rv);
-#pragma unroll
-                for (int i = 0; i < C; ++i) {
-                    const double fac = n_alpha - jap1[j + i];
-                    acc = vfma(splat<N>(fac), rv[C - 1 - i] * qv[i], acc);
-                }
-            }
-            for (; j < n; ++j) {
-                tm::words<2 * N> wq, wr;
-                Q.template issue<1>(j, wq);
-                R2.template issue<1>(n - j, wr);
-                tm::wait_ld(wq);
-                tm::wait_ld(wr);
-                V qv[1], rv[1];
-                TRow::template unpack<1>(wq, qv);
-                TRow::template unpack<1>(wr, rv);
-                const double fac = n_alpha - jap1[j];
-                acc = vfma(splat<N>(fac), rv[0] * qv[0], acc);
-            }
-            tm::wait_ld(w0);
-            V r20[1];
-            TRow::template unpack<1>(w0, r20);
-            q = acc / (nd * r20[0]);
-        }
-        Q.set(n, q);
-
-        // q descending, d ascending.
-        const double *pd0 = d0[0], *pd1 = d0[1], *pd2 = TD == 0 ? d0[2] : nullptr;
-        std::uint32_t j = 0;
-        for (; j + C <= n + 1u; j += C) {
-            V qv[C], dv[C];
-            ldc(Q, n - j - (C - 1u), qv); // q^[n - j - i] = qv[C - 1 - i]
-            if constexpr (TD == 1) {
-                ldc(D2, j, dv);
-            }
-#pragma unroll
-            for (int i = 0; i < C; ++i) {
-                const V fj = c1 * qv[C - 1 - i];
-                acc[0] = vfma(fj, Row::load(pd0), acc[0]);
-                acc[1] = vfma(fj, Row::load(pd1), acc[1]);
-                acc[2] = vfma(fj, TD == 1 ? dv[i] : Row::load(pd2), acc[2]);
-                pd0 += S;
-                pd1 += S;
-                if (TD == 0) {
-                    pd2 += S;
-                }
-            }
-        }
-        for (; j <= n; ++j) {
-            const V fj = c1 * Q.get(n - j);
-            acc[0] = vfma(fj, Row::load(pd0), acc[0]);
-            acc[1] = vfma(fj, Row::load(pd1), acc[1]);
-            acc[2] = vfma(fj, TD == 1 ? D2.get(j) : Row::load(pd2), acc[2]);
-            pd0 += S;
-            pd1 += S;
-            if (TD == 0) {
-                pd2 += S;
-            }
-        }
-    }
-    if (active) {
-#pragma unroll
-        for (int k = 0; k < 3; ++k) {
-            Row::store(const_cast<double *>(t.hrow(aux[15 + 4 * k]).hptr(0u)), acc[k]);
-            if (aux[27 + k] != 0u) {
-                sv_out(aux[27 + k], acc[k], n);
-            }
-            if (have_n) {
-                const V nk = t.cst(aux[18 + 4 * k]) * acc[k];
-                Row::store(const_cast<double *>(t.hrow(aux[17 + 4 * k]).hptr(0u)), nk);
-                if (aux[30 + k] != 0u) {
-                    sv_out(aux[30 + k], nk, n);
-                }
             }
         }
     }

@@ -1,4 +1,4 @@
-// The sm_100a kernels of the batch Taylor integrator.
+// The sm_90a kernels of the batch Taylor integrator.
 //
 // k_coop (the product path): warp-cooperative. A warp owns L lanes and their compact derivative tape ([slot][L]
 //   doubles; only what is re-read at later orders keeps its history, see smem_plan.hpp). Its 32 threads share the
@@ -9,7 +9,6 @@
 //   atomic counter and run a group's whole propagate_until() loop in one go; they never wait for each other.
 //   Where the tape lives is the kernel's MODE:
 //     0 / 1  shared memory (0: superinstruction-only programs, no interpreter of the elementary recurrences);
-//     2 / 3  shared memory + tensor memory for the rows only one thread touches (tmem.cuh);
 //     4 / 5  a slab of global memory per team, tables read in place (systems too large for shared memory);
 //            4: a team is a warp, 5: a team is the whole CTA (wide levels, few lanes; see team<>).
 //   HBM traffic per step: the state in and out (the state variables' coefficients go to a private L2-resident
@@ -428,7 +427,7 @@ struct coop_header {
     std::uint32_t off_ops, off_seg, off_args, off_aux;
     std::uint32_t off_consts, off_sv, n_slots, off_svout;
     std::uint32_t off_svphase, n_svphase, off_rcp, n_gslots;
-    std::uint32_t tmem, reserved0, reserved1, reserved2; // tmem: rows per pair interaction kept in TMEM (0, 2, 3)
+    std::uint32_t reserved0, reserved1, reserved2, reserved3;
 };
 
 template <int L, int N>
@@ -619,16 +618,13 @@ struct sv_writer {
 
 // Jet of the L lanes starting at global lane `lane0`; the state variables' coefficients go to tc.
 // MODE: 1 = the program contains elementary ops; 0 = superinstructions only (the interpreter of the elementary
-// recurrences is compiled out, which keeps the hot code small); 2 / 3 = superinstructions only, with two / three
-// private history rows of the pair interactions in tensor memory (tm_r2 = TMEM address of this warp's columns):
-// level 0 then consists of at most 32 / G pair interactions, one per thread, run by the whole warp, converged.
+// recurrences is compiled out, which keeps the hot code small); 4 / 5 = tape in global memory.
 template <int L, int N, int MODE>
 __device__ __forceinline__ void coop_jet(const program &P, const coop_header &H, const std::uint32_t *tab,
                                          const batch &D, const coop_smem<L> &S, std::uint32_t lane0, double *gtape,
-                                         std::uint32_t tm_r2, const coef_view &cv)
+                                         const coef_view &cv)
 {
     constexpr bool GEN = MODE == 1 || MODE == 4 || MODE == 5;
-    constexpr bool TMEM = MODE == 2 || MODE == 3;
     using T = team<MODE == 5>;
     constexpr std::uint32_t G = L / N; // lane groups per warp
     const std::uint32_t tid = T::tid();
@@ -667,31 +663,6 @@ __device__ __forceinline__ void coop_jet(const program &P, const coop_header &H,
     }
     const sv_writer<L, N> &sv_out = sv_out_;
     const auto write_tc = [&](std::uint32_t sv, std::uint32_t n, const vd<N> &v) { sv_out.write_tc(sv, n, v); };
-
-    // Tensor-memory modes run the pair level with one pair interaction per thread (N lanes each); the levels after
-    // it (sums of the pairs' outputs, a handful of items) are run with NS >= N lanes per thread, so that e.g. the
-    // 18 sums x 2 lanes of the 6-body system are one round of 18 threads instead of 32 + 4. A slot holds the L
-    // lanes of the warp contiguously, so the two views of the tape differ only in the lanes a thread touches.
-    constexpr int NS = (TMEM && N == 1 && L >= 2) ? 2 : N;
-    constexpr std::uint32_t GS = L / NS;
-    smem_tape<L, NS> ts;
-    const std::uint32_t gs = tid % GS;
-    ts.base = S.tape + gs * NS;
-    ts.gbase = nullptr;
-    ts.args = t.args;
-    ts.consts = t.consts;
-    ts.pars = D.pars;
-    ts.batch = D.n;
-    sv_writer<L, NS> sv_out_s_{ts, cv, svout, rcp, p, {}, {}};
-#pragma unroll
-    for (int i = 0; i < NS; ++i) {
-        const std::uint32_t l = lane0 + gs * NS + i;
-        sv_out_s_.lane_ok[i] = l < D.n && !(cv.mask_idle && S.running[gs * NS + i] == 0);
-        ts.glane[i] = l < D.n ? l : D.n - 1u;
-        ts.tm.v[i] = S.time[gs * NS + i];
-        sv_out_s_.loff[i] = cv.lane_off(ts.glane[i], gs * NS + i);
-    }
-    const sv_writer<L, NS> &sv_out_s = sv_out_s_;
 
     // Order 0 of the state variables: the state itself; order 1 of those that derive from another state
     // variable (x^[1] = v^[0]). (it % G == g because nthr is a multiple of G.)
@@ -738,28 +709,6 @@ __device__ __forceinline__ void coop_jet(const program &P, const coop_header &H,
         // The other u variables, one dependency level at a time.
         for (std::uint32_t s = 0; s < H.n_segments; ++s) {
             const std::uint32_t b = seg[s], e = seg[s + 1u];
-            if constexpr (TMEM) {
-                if (s == 0u) {
-                    const std::uint32_t cnt = (e - b) * G;
-                    const bool active = tid < cnt;
-                    const uint4 op = ops[2u * (b + (active ? tid : cnt - 1u) / G)];
-                    fused_nbody_pair_tmem<N, TMEM ? MODE - 2 : 0>(P, t, aux + op.y, op.z, op.w != 0u, n, sv_out, active, tm_r2);
-                    T::sync();
-                    continue;
-                }
-                // The other levels of a superinstruction-only program: sums of single-slot rows.
-                for (std::uint32_t it = tid; it < (e - b) * GS; it += nthr) {
-                    const std::uint32_t k = b + it / GS;
-                    const uint4 op = ops[2u * k], op2 = ops[2u * k + 1u];
-                    const vd<NS> v = sum_single_slot<NS>(ts, op.y, op.z);
-                    ts.row(op2.x).set(n, v);
-                    if (op2.y != 0u) {
-                        sv_out_s(op2.y, v, n);
-                    }
-                }
-                T::sync();
-                continue;
-            }
             for (std::uint32_t it = tid; it < (e - b) * G; it += nthr) {
                 const std::uint32_t k = b + it / G;
                 const uint4 op = ops[2u * k];
@@ -874,7 +823,6 @@ template <int L, int N, bool PROP, int MAXT, int MODE>
 __global__ void __launch_bounds__(MAXT, 1)
     k_coop(program P, const std::uint32_t *blob, batch D, run_args R, double *gscratch)
 {
-    constexpr bool TMEM = MODE == 2 || MODE == 3;
     // MODE 4: systems whose compact tape does not fit in shared memory. Same kernel, but the warp's tape lives in
     // a per-warp slab of global memory (gscratch) and the program tables are read in place (L1 / L2).
     constexpr bool GLOBAL = MODE == 4 || MODE == 5;
@@ -892,23 +840,7 @@ __global__ void __launch_bounds__(MAXT, 1)
         }
         tab = stab;
     }
-    // Tensor memory: warp 0 allocates all the columns; warp w then owns the columns [(w / 4) * cols, ...) of the
-    // 32 TMEM lanes of its quadrant w % 4, one TMEM lane per thread (tmem.cuh).
-    __shared__ std::uint32_t tm_base_smem;
-    std::uint32_t tm_r2 = 0u;
-    if constexpr (TMEM) {
-        if ((threadIdx.x >> 5) == 0u) {
-            tm::alloc_all(&tm_base_smem);
-        }
-        tm::fence_before_sync();
-    }
     __syncthreads();
-    if constexpr (TMEM) {
-        tm::fence_after_sync();
-        const std::uint32_t w = threadIdx.x >> 5;
-        const std::uint32_t cols_per_warp = static_cast<std::uint32_t>(MODE) * (P.order + 1u) * tm::row<N>::W;
-        tm_r2 = tm_base_smem + (((w & 3u) * 32u) << 16) + (w >> 2) * cols_per_warp;
-    }
     const coop_header H = *reinterpret_cast<const coop_header *>(tab);
 
     const std::uint32_t tid = T::tid();
@@ -952,7 +884,7 @@ __global__ void __launch_bounds__(MAXT, 1)
                 S.running[tid] = skipped ? 0 : 1;
             }
             T::sync();
-            coop_jet<L, N, MODE>(P, H, tab, D, S, lane0, gtape, tm_r2, cv);
+            coop_jet<L, N, MODE>(P, H, tab, D, S, lane0, gtape, cv);
             const double h = (!CTA || threadIdx.x < 32u) ? coop_determine_h<L>(P, D, cv, lane0, mdt) : 0.;
             if (owner) {
                 S.h[tid] = h;
@@ -984,7 +916,7 @@ __global__ void __launch_bounds__(MAXT, 1)
                     S.running[tid] = lp.running ? 1 : 0;
                 }
                 T::sync();
-                coop_jet<L, N, MODE>(P, H, tab, D, S, lane0, gtape, tm_r2, cv);
+                coop_jet<L, N, MODE>(P, H, tab, D, S, lane0, gtape, cv);
                 const double h = (!CTA || threadIdx.x < 32u) ? coop_determine_h<L>(P, D, cv, lane0, cur_max) : 0.;
                 if (owner) {
                     S.h[tid] = h;
@@ -1003,13 +935,6 @@ __global__ void __launch_bounds__(MAXT, 1)
             }
         }
         T::sync();
-    }
-    if constexpr (TMEM) {
-        tm::fence_before_sync();
-        __syncthreads();
-        if ((threadIdx.x >> 5) == 0u) {
-            tm::dealloc_all(tm_base_smem);
-        }
     }
 }
 

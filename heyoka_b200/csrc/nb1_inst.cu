@@ -8,13 +8,13 @@ namespace heyoka_b200::detail
 namespace
 {
 
-#define HY_NB1(TM, MAXT)                                                                                               \
+#define HY_NB1(MAXT)                                                                                                   \
     nb_variant                                                                                                         \
     {                                                                                                                  \
-        32, false, TM, MAXT, dev::k_nb1<TM, false, MAXT>, dev::k_nb1<TM, true, MAXT>, true                             \
+        32, false, false, MAXT, dev::k_nb1<false, false, MAXT>, dev::k_nb1<false, true, MAXT>, true                    \
     }
 
-const nb_variant family[] = {HY_NB1(true, 512), HY_NB1(true, 384), HY_NB1(true, 256), HY_NB1(false, 512), HY_NB1(false, 256)};
+const nb_variant family[] = {HY_NB1(512), HY_NB1(384), HY_NB1(256)};
 
 } // namespace
 

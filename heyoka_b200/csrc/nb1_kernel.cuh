@@ -39,9 +39,9 @@ namespace nbk
 {
 
 // pair_block()'s storage policy for a thread that owns its lane: positions in, pair outputs out are registers; the
-// private history rows are those of pair_mem<32, TMEM>.
-template <bool TMEM>
-struct pair_mem1 : pair_mem<32, TMEM> {
+// private history rows are those of pair_mem<32, OFFCHIP>.
+template <bool OFFCHIP>
+struct pair_mem1 : pair_mem<32, OFFCHIP> {
     d2 xa[3], xb[3];   // (x^[n], x^[n+1]) of the two bodies
     d2 om_[3], on_[3]; // (m_k^[n], m_k^[n+1]), (n_k^[n], n_k^[n+1])
 
@@ -82,7 +82,7 @@ __device__ __forceinline__ double nb1_div(double x, std::uint32_t n, double nd, 
     return x == 0. ? x : nb::div_cold(x, nd);
 }
 
-template <bool TMEM, bool PROP, int MAXT>
+template <bool OFFCHIP, bool PROP, int MAXT>
 __global__ void __launch_bounds__(MAXT, 1) k_nb1(program P, nb_dev_plan NP, batch D, run_args R)
 {
     using nb::d2;
@@ -108,18 +108,12 @@ __global__ void __launch_bounds__(MAXT, 1) k_nb1(program P, nb_dev_plan NP, batc
     for (std::uint32_t i = threadIdx.x; i < n_rcp; i += blockDim.x) {
         rcp_s[i] = i == 0u ? 0. : 1. / static_cast<double>(i);
     }
-    __shared__ std::uint32_t tm_base_smem;
-    if constexpr (TMEM) {
-        if ((threadIdx.x >> 5) == 0u) {
-            tm::alloc_all(&tm_base_smem);
-        }
-        tm::fence_before_sync();
-    }
+    static_assert(!OFFCHIP, "the one-thread-per-lane kernel keeps its private rows in shared memory");
     __syncthreads();
 
     const std::uint32_t tid = threadIdx.x & 31u, warp = threadIdx.x >> 5;
     double *region = smem_raw + NP.shared_doubles + static_cast<std::size_t>(warp) * NP.team_doubles;
-    using PM_t = nbk::pair_mem1<TMEM>;
+    using PM_t = nbk::pair_mem1<OFFCHIP>;
     PM_t PM;
     nb::pair_consts PC;
     {
@@ -136,11 +130,7 @@ __global__ void __launch_bounds__(MAXT, 1) k_nb1(program P, nb_dev_plan NP, batc
         PM.fac_ = nbk::saddr(fac_s);
         PM.fac_stride_b = NP.fac_stride * 8u;
         PM.flags = 0u;
-        PM.tmc = 0u;
-        if constexpr (TMEM) {
-            tm::fence_after_sync();
-            PM.tmc = tm_base_smem + (((warp & 3u) * 32u) << 16) + (warp >> 2) * (NP.npp * 12u);
-        }
+        PM.grow = nullptr;
 #pragma unroll
         for (int k = 0; k < 3; ++k) {
             PM.on_[k] = d2{0., 0.};
@@ -177,11 +167,8 @@ __global__ void __launch_bounds__(MAXT, 1) k_nb1(program P, nb_dev_plan NP, batc
         }
         double *vp = cb; // V(n + 1, 0)
         for (std::uint32_t m = 0; m < n_blocks; ++m) {
-            __syncwarp(); // (the tensor-memory accesses of pair_block() are warp-wide: converged)
+            __syncwarp();
             nb::pair_block(PM, PC, m);
-            if constexpr (TMEM) {
-                tm::wait_st();
-            }
             const std::uint32_t n = 2u * m;
             const double n1 = static_cast<double>(n + 1u), n2 = static_cast<double>(n + 2u),
                          n3 = static_cast<double>(n + 3u);
@@ -454,13 +441,6 @@ __global__ void __launch_bounds__(MAXT, 1) k_nb1(program P, nb_dev_plan NP, batc
             }
         }
         __syncwarp();
-    }
-    if constexpr (TMEM) {
-        tm::fence_before_sync();
-        __syncthreads();
-        if ((threadIdx.x >> 5) == 0u) {
-            tm::dealloc_all(tm_base_smem);
-        }
     }
 }
 

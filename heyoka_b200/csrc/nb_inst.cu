@@ -16,18 +16,18 @@ namespace heyoka_b200::detail
 namespace
 {
 
-#define HY_NB(TM, MAXT)                                                                                                \
+#define HY_NB(OFF, MAXT)                                                                                               \
     nb_variant                                                                                                         \
     {                                                                                                                  \
-        HY_NB_LT, HY_NB_CTA != 0, TM, MAXT, dev::k_nb<HY_NB_LT, HY_NB_CTA != 0, TM, false, MAXT>,                      \
-            dev::k_nb<HY_NB_LT, HY_NB_CTA != 0, TM, true, MAXT>                                                        \
+        HY_NB_LT, HY_NB_CTA != 0, OFF, MAXT, dev::k_nb<HY_NB_LT, HY_NB_CTA != 0, OFF, false, MAXT>,                    \
+            dev::k_nb<HY_NB_LT, HY_NB_CTA != 0, OFF, true, MAXT>                                                       \
     }
 
 const nb_variant family[] = {
 #if HY_NB_CTA != 0
-    HY_NB(true, 512), HY_NB(false, 512)
+    HY_NB(false, 512), HY_NB(true, 512)
 #else
-    HY_NB(true, 512), HY_NB(true, 384), HY_NB(true, 256), HY_NB(false, 512), HY_NB(false, 256)
+    HY_NB(false, 512), HY_NB(false, 384), HY_NB(false, 256)
 #endif
 };
 

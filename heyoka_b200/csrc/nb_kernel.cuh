@@ -1,4 +1,4 @@
-// k_nb: the dedicated sm_100a kernel for N-body-shaped programs (nb_plan.hpp): model::nbody of the outer Solar System
+// k_nb: the dedicated sm_90a kernel for N-body-shaped programs (nb_plan.hpp): model::nbody of the outer Solar System
 // (6 bodies, 15 pair interactions), the two-body step benchmark, model::nbody with 32 bodies (496 pair interactions).
 //
 // Same persistent structure as k_coop (kernels.cuh): a team (a warp, or the whole CTA when one lane has hundreds of pair
@@ -8,10 +8,10 @@
 //   * the orders are walked two at a time (nb_core.hpp), two synchronisations per PAIR of orders;
 //   * a thread is bound to one (pair interaction, lane) for the whole kernel: its operands' shared-memory addresses
 //     and constants live in registers, nothing is decoded per order;
-//   * its private history rows are stored as (even order, odd order) pairs: d_0, d_1 in shared memory, interleaved by
-//     thread ([order pair][row][thread], one 16-byte access per thread, conflict-free), r^2, d_2 and r^alpha in tensor
-//     memory (12 columns per order pair: one tcgen05.ld.x8 + one .x4 per loop iteration); or all five in shared
-//     memory (TMEM = false);
+//   * its private history rows are stored as (even order, odd order) pairs in shared memory, interleaved by thread
+//     ([order pair][row][thread], one 16-byte access per thread, conflict-free); with CTA teams, when the five rows of
+//     512 threads do not fit in shared memory (model::nbody with 32 bodies), r^2, d_2 and r^alpha go to a per-CTA
+//     slab of global memory that stays in L2 (OFFCHIP = true; same interleaving, coalesced);
 //   * shared memory otherwise only holds what threads exchange: the positions of the current order pair and the
 //     outputs of the pair interactions / partial sums ([role][pair][lane] so that a warp writes consecutive slots);
 //   * what a thread does in the summation phase is a pre-decoded 32-byte record (nb_role) per round;
@@ -31,7 +31,6 @@
 #include "kernels.cuh"
 #include "nb_core.hpp"
 #include "nb_desc.hpp"
-#include "tmem.cuh"
 
 namespace heyoka_b200::dev
 {
@@ -58,6 +57,7 @@ struct nb_dev_plan {
     std::uint32_t shared_doubles; // CTA-shared tables: fac | rcp | consts | roles
     std::uint32_t team_doubles;   // per team: positions | outputs | private rows | norms | scalars
     std::uint32_t n_slots_equiv;  // team region (without the scalars) expressed in coop_smem<LT> slots
+    double *offchip;              // OFFCHIP kernels: per CTA, [order pair][3 rows][thread] pairs of doubles
     nb1_tab l1;                   // k_nb1 only
 };
 
@@ -107,32 +107,32 @@ __device__ __forceinline__ d2 from_words(std::uint32_t a, std::uint32_t b, std::
     return d2{__hiloint2double(static_cast<int>(b), static_cast<int>(a)),
               __hiloint2double(static_cast<int>(d), static_cast<int>(c))};
 }
-__device__ __forceinline__ tm::words<4> to_words(const d2 &v)
-{
-    tm::words<4> w;
-    w.w[0] = static_cast<std::uint32_t>(__double2loint(v.x));
-    w.w[1] = static_cast<std::uint32_t>(__double2hiint(v.x));
-    w.w[2] = static_cast<std::uint32_t>(__double2loint(v.y));
-    w.w[3] = static_cast<std::uint32_t>(__double2hiint(v.y));
-    return w;
-}
 
 // Storage policy of pair_block() (nb_core.hpp). TT = threads per team. All members are shared-window addresses.
 // Private rows in shared memory: element (order pair op, row r) of this thread at drow + (op * NSR + r) * TT * 16,
-// rows d_0, d_1 (+ d_2, r^2, r^alpha when TMEM is false). Tensor memory: columns [op * 12, op * 12 + 12) of the
-// thread's TMEM lane = r^2 pair, d_2 pair, r^alpha pair.
-template <int TT, bool TMEM>
+// rows d_0, d_1 (+ d_2, r^2, r^alpha when OFFCHIP is false). Off chip: element (op, r) of this thread at
+// grow[(op * 3 + r) * TT], rows r^2, d_2, r^alpha.
+template <int TT, bool OFFCHIP>
 struct pair_mem {
-    static constexpr int NSR = TMEM ? 2 : 5;
+    static constexpr int NSR = OFFCHIP ? 2 : 5;
     static constexpr std::uint32_t OPB = static_cast<std::uint32_t>(NSR) * TT * 16u; // bytes per order pair
     static constexpr std::uint32_t RB = TT * 16u;                                    // bytes per row
     std::uint32_t pa[3], pb[3]; // the six positions this pair reads (this thread's lane)
     std::uint32_t om, kstride;  // output m_0 of this (pair, lane); m_k / n_k are k / (3 + k) strides further
     std::uint32_t drow;         // this thread's slice of the private rows
     std::uint32_t fac_, fac_stride_b;
-    std::uint32_t tmc; // TMEM address of this thread's column 0
+    double2 *grow; // OFFCHIP: this thread's element (0, 0)
     std::uint32_t flags; // bit 0: active (owns a pair), bits 1-3: n_k exists
 
+    __device__ __forceinline__ d2 gld(std::uint32_t op, std::uint32_t r) const
+    {
+        const double2 v = grow[(op * 3u + r) * TT];
+        return d2{v.x, v.y};
+    }
+    __device__ __forceinline__ void gst(std::uint32_t op, std::uint32_t r, const d2 &v) const
+    {
+        grow[(op * 3u + r) * TT] = make_double2(v.x, v.y);
+    }
     __device__ __forceinline__ d2 pos_a(int k) const
     {
         return lds2(pa[k]);
@@ -146,24 +146,24 @@ struct pair_mem {
         const std::uint32_t p = drow + m * OPB;
         sts2(p, D[0]);
         sts2(p + RB, D[1]);
-        if constexpr (TMEM) {
-            tm::st(tmc + m * 12u + 4u, to_words(D[2]));
+        if constexpr (OFFCHIP) {
+            gst(m, 1u, D[2]);
         } else {
             sts2(p + 2u * RB, D[2]);
         }
     }
     __device__ __forceinline__ void st_r2(std::uint32_t m, const d2 &r) const
     {
-        if constexpr (TMEM) {
-            tm::st(tmc + m * 12u, to_words(r));
+        if constexpr (OFFCHIP) {
+            gst(m, 0u, r);
         } else {
             sts2(drow + m * OPB + 3u * RB, r);
         }
     }
     __device__ __forceinline__ void st_q(std::uint32_t m, const d2 &q) const
     {
-        if constexpr (TMEM) {
-            tm::st(tmc + m * 12u + 8u, to_words(q));
+        if constexpr (OFFCHIP) {
+            gst(m, 2u, q);
         } else {
             sts2(drow + m * OPB + 4u * RB, q);
         }
@@ -171,18 +171,13 @@ struct pair_mem {
     __device__ __forceinline__ void ld_ss(std::uint32_t ai, std::uint32_t li, d2 (&A)[3], d2 (&Lo)[3]) const
     {
         const std::uint32_t pa_ = drow + ai * OPB, pl = drow + li * OPB;
-        if constexpr (TMEM) {
-            tm::words<4> wa, wl;
-            tm::ld(tmc + ai * 12u + 4u, wa);
-            tm::ld(tmc + li * 12u + 4u, wl);
+        if constexpr (OFFCHIP) {
+            A[2] = gld(ai, 1u);
+            Lo[2] = gld(li, 1u);
             A[0] = lds2(pa_);
             A[1] = lds2(pa_ + RB);
             Lo[0] = lds2(pl);
             Lo[1] = lds2(pl + RB);
-            tm::wait_ld(wa);
-            tm::wait_ld(wl);
-            A[2] = from_words(wa.w[0], wa.w[1], wa.w[2], wa.w[3]);
-            Lo[2] = from_words(wl.w[0], wl.w[1], wl.w[2], wl.w[3]);
         } else {
 #pragma unroll
             for (int k = 0; k < 3; ++k) {
@@ -194,13 +189,10 @@ struct pair_mem {
     __device__ __forceinline__ void ld_a(std::uint32_t ai, d2 (&A)[3]) const
     {
         const std::uint32_t pa_ = drow + ai * OPB;
-        if constexpr (TMEM) {
-            tm::words<4> wa;
-            tm::ld(tmc + ai * 12u + 4u, wa);
+        if constexpr (OFFCHIP) {
+            A[2] = gld(ai, 1u);
             A[0] = lds2(pa_);
             A[1] = lds2(pa_ + RB);
-            tm::wait_ld(wa);
-            A[2] = from_words(wa.w[0], wa.w[1], wa.w[2], wa.w[3]);
         } else {
 #pragma unroll
             for (int k = 0; k < 3; ++k) {
@@ -211,18 +203,12 @@ struct pair_mem {
     __device__ __forceinline__ void ld_main(std::uint32_t qi, std::uint32_t li, d2 &Q, d2 &Rlo, d2 (&Dlo)[3]) const
     {
         const std::uint32_t pl = drow + li * OPB;
-        if constexpr (TMEM) {
-            tm::words<8> wl;
-            tm::words<4> wq;
-            tm::ld(tmc + li * 12u, wl);
-            tm::ld(tmc + qi * 12u + 8u, wq);
+        if constexpr (OFFCHIP) {
+            Rlo = gld(li, 0u);
+            Dlo[2] = gld(li, 1u);
+            Q = gld(qi, 2u);
             Dlo[0] = lds2(pl);
             Dlo[1] = lds2(pl + RB);
-            tm::wait_ld(wl);
-            tm::wait_ld(wq);
-            Rlo = from_words(wl.w[0], wl.w[1], wl.w[2], wl.w[3]);
-            Dlo[2] = from_words(wl.w[4], wl.w[5], wl.w[6], wl.w[7]);
-            Q = from_words(wq.w[0], wq.w[1], wq.w[2], wq.w[3]);
         } else {
 #pragma unroll
             for (int k = 0; k < 3; ++k) {
@@ -397,10 +383,11 @@ static __device__ __noinline__ double nb_step_size(const program &P, unsigned lo
     return h_from_norms(P, isnan(f0) ? f0 : m0, isnan(fp) ? fp : mp, isnan(fp1) ? fp1 : mp1, max_delta_t);
 }
 
-// LT: lanes per team; CTA: a team is the whole CTA (else a warp); TMEM: r^2, d_2, r^alpha rows in tensor memory.
-template <int LT, bool CTA, bool TMEM, bool PROP, int MAXT>
+// LT: lanes per team; CTA: a team is the whole CTA (else a warp); OFFCHIP: r^2, d_2, r^alpha rows in NP.offchip.
+template <int LT, bool CTA, bool OFFCHIP, bool PROP, int MAXT>
 __global__ void __launch_bounds__(MAXT, 1) k_nb(program P, nb_dev_plan NP, batch D, run_args R)
 {
+    static_assert(!OFFCHIP || CTA, "off-chip private rows are laid out per CTA");
     using T = team<CTA>;
     constexpr int TT = CTA ? MAXT : 32; // threads per team (CTA teams are launched with exactly MAXT threads)
     constexpr int NL = LT >= 2 ? 2 : 1; // lanes per thread in the summation phase
@@ -430,13 +417,6 @@ __global__ void __launch_bounds__(MAXT, 1) k_nb(program P, nb_dev_plan NP, batch
             roles_s[i] = __ldg(NP.roles + i);
         }
     }
-    __shared__ std::uint32_t tm_base_smem;
-    if constexpr (TMEM) {
-        if ((threadIdx.x >> 5) == 0u) {
-            tm::alloc_all(&tm_base_smem);
-        }
-        tm::fence_before_sync();
-    }
     __syncthreads();
 
     const std::uint32_t tid = T::tid();
@@ -446,20 +426,20 @@ __global__ void __launch_bounds__(MAXT, 1) k_nb(program P, nb_dev_plan NP, batch
     std::uint32_t pos_b = nbk::saddr(region);
     std::uint32_t out_b = pos_b + NP.n_pos * LT * 16u;
     const std::uint32_t drow_b = out_b + NP.n_out * LT * 16u;
-    const std::uint32_t norms_b = drow_b + NP.npp * nbk::pair_mem<TT, TMEM>::OPB;
+    const std::uint32_t norms_b = drow_b + NP.npp * nbk::pair_mem<TT, OFFCHIP>::OPB;
     nbk::keep(pos_b);
     nbk::keep(out_b);
     unsigned long long *norms_p
         = reinterpret_cast<unsigned long long *>(region + (static_cast<std::size_t>(NP.n_pos) + NP.n_out) * LT * 2u
-                                                 + static_cast<std::size_t>(NP.npp) * nbk::pair_mem<TT, TMEM>::OPB / 8u);
+                                                 + static_cast<std::size_t>(NP.npp) * nbk::pair_mem<TT, OFFCHIP>::OPB / 8u);
 
     // ---- this thread's pair interaction ----
-    nbk::pair_mem<TT, TMEM> PM;
+    nbk::pair_mem<TT, OFFCHIP> PM;
     nb::pair_consts PC;
     {
         const std::uint32_t n_pt = NP.n_pairs * LT;
         const bool active = tid < n_pt;
-        // Idle threads shadow pair 0 / lane 0 on their own private rows (the tensor-memory accesses are warp-wide).
+        // Idle threads shadow pair 0 / lane 0 (they skip the pair phase).
         const std::uint32_t pi = active ? tid / LT : 0u, l = active ? tid % LT : 0u;
         const uint4 *dp = reinterpret_cast<const uint4 *>(NP.pairs + pi);
         const uint4 w0 = __ldg(dp), w1 = __ldg(dp + 1), w2 = __ldg(dp + 2), w3 = __ldg(dp + 3);
@@ -490,12 +470,10 @@ __global__ void __launch_bounds__(MAXT, 1) k_nb(program P, nb_dev_plan NP, batch
         PM.drow = drow_b + tid * 16u;
         PM.fac_ = nbk::saddr(fac_s);
         PM.fac_stride_b = NP.fac_stride * 8u;
-        PM.tmc = 0u;
-        if constexpr (TMEM) {
-            tm::fence_after_sync();
-            // Warp w owns the columns [(w / 4) * cols, ...) of the 32 TMEM lanes of its quadrant w % 4.
-            const std::uint32_t w = threadIdx.x >> 5;
-            PM.tmc = tm_base_smem + (((w & 3u) * 32u) << 16) + (w >> 2) * (NP.npp * 12u);
+        PM.grow = nullptr;
+        if constexpr (OFFCHIP) {
+            PM.grow = reinterpret_cast<double2 *>(NP.offchip)
+                      + static_cast<std::size_t>(blockIdx.x) * NP.npp * 3u * TT + threadIdx.x;
         }
     }
     // ---- this thread's lanes in the summation phase ----
@@ -562,11 +540,8 @@ __global__ void __launch_bounds__(MAXT, 1) k_nb(program P, nb_dev_plan NP, batch
         }
         T::sync();
         for (std::uint32_t m = 0; m < n_blocks; ++m) {
-            if (TMEM || (PM.flags & 1u) != 0u) {
+            if ((PM.flags & 1u) != 0u) {
                 nb::pair_block(PM, PC, m);
-            }
-            if constexpr (TMEM) {
-                tm::wait_st();
             }
             T::sync();
             RM.track = m + 2u >= n_blocks;
@@ -668,13 +643,6 @@ __global__ void __launch_bounds__(MAXT, 1) k_nb(program P, nb_dev_plan NP, batch
             }
         }
         T::sync();
-    }
-    if constexpr (TMEM) {
-        tm::fence_before_sync();
-        __syncthreads();
-        if ((threadIdx.x >> 5) == 0u) {
-            tm::dealloc_all(tm_base_smem);
-        }
     }
 }
 

@@ -1,7 +1,7 @@
-// k_nn: the sm_100a kernel for right-hand sides that are dense feed-forward networks, x' = ffnn(x) (nn_plan.hpp;
+// k_nn: the sm_90a kernel for right-hand sides that are dense feed-forward networks, x' = ffnn(x) (nn_plan.hpp;
 // BASELINE.json configs[4]: model::ffnn, 3 x 64 tanh, order 15).
 //
-// A CTA of 256 threads owns LB = 3 lanes and runs their whole propagate_until() loop (persistent, chunks claimed from
+// A CTA of 256 threads owns LB = 2 lanes and runs their whole propagate_until() loop (persistent, chunks claimed from
 // an atomic counter, like k_coop / k_nb). Per Taylor order n and layer:
 //   * the layer's linear part z^[n] = W a^[n] (+ b at order 0) is ONE matrix product [n_out x n_in] . [n_in x lanes] on
 //     the FP64 tensor cores: mma.sync.aligned.m8n8k4.f64 (SASS DMMA), 8 output neurons per warp and instruction, the
@@ -9,11 +9,10 @@
 //   * the weights of every layer are staged ONCE per CTA from global to shared memory by the TMA unit (one
 //     cp.async.bulk + mbarrier of the host-prepared, bank-conflict-free padded image: SASS UBLKCP), and stay there;
 //   * tanh (src/math/tanh.cpp:183-318) and its hidden dependency tanh^2 (src/math/pow.cpp square recurrence) are run by
-//     one thread per (neuron, lane) with the reference's sequential summation order. The histories of z and tanh, which
-//     other threads write / read, are [row][order][neuron][lane] arrays in shared memory; the history of tanh^2, which
-//     only its own thread ever touches, lives in TENSOR MEMORY (48 columns per (neuron, lane, layer), read back eight
-//     orders at a time with tcgen05.ld.x16): a third of the history bytes leaves shared memory, which is what bounds the
-//     lanes per CTA (3 instead of 2);
+//     one thread per (neuron, lane) with the reference's sequential summation order. The histories of z, tanh and
+//     tanh^2 are [row][order][neuron][lane] arrays in shared memory (tanh^2 is only ever touched by its own thread).
+//     The histories are what bounds the lanes per CTA: 3 x 64 tanh at order 15 takes 2 lanes in the 227 KB of an
+//     H100 SM;
 //   * the output layer's z^[n] are the derivatives of the state variables: x^[n+1] = z^[n] / (n + 1).
 // The Taylor coefficients of the state variables live in shared memory too (step size, state update, optional copy to
 // the public tc array): apart from state in / state out nothing touches HBM.
@@ -27,13 +26,12 @@
 #include <cuda_runtime.h>
 
 #include "kernels.cuh"
-#include "tmem.cuh"
 
 namespace heyoka_b200::dev
 {
 
 constexpr int NN_MAX_LAYERS = 8;
-constexpr int NN_LB = 3;        // lanes per CTA
+constexpr int NN_LB = 2;        // lanes per CTA
 constexpr int NN_THREADS = 256; // 8 warps
 
 struct nn_dev_plan {
@@ -44,11 +42,8 @@ struct nn_dev_plan {
     std::uint32_t n_in[NN_MAX_LAYERS], n_out[NN_MAX_LAYERS], act[NN_MAX_LAYERS];
     std::uint32_t n_in_pad[NN_MAX_LAYERS], n_out_pad[NN_MAX_LAYERS]; // multiples of 4 / 8
     std::uint32_t ldw[NN_MAX_LAYERS], w_off[NN_MAX_LAYERS], b_off[NN_MAX_LAYERS]; // doubles, into wimg
-    std::uint32_t hist_off[NN_MAX_LAYERS]; // doubles, into the history area: [2][order][n_out][LB] (hidden layers)
+    std::uint32_t hist_off[NN_MAX_LAYERS]; // doubles, into the history area: [3][order][n_out][LB] (hidden layers)
     std::uint32_t hist_doubles, max_out;
-    // Tensor memory: thread t keeps the tanh^2 history of its r-th (neuron, lane) item of hidden layer L in the 48
-    // columns starting at (tm_slot[L] * tm_ipt + r) * 48 of its region (256 columns per thread: 2 warps per quadrant).
-    std::uint32_t tm_ipt, tm_slot[NN_MAX_LAYERS];
 };
 
 namespace nnk
@@ -114,17 +109,10 @@ __global__ void __launch_bounds__(NN_THREADS, 1) k_nn(program P, nn_dev_plan NP,
     __shared__ __align__(8) std::uint64_t wbar;
     __shared__ unsigned int claimed;
     __shared__ lane_prop parked[LB];
-    __shared__ std::uint32_t tm_base_smem;
     __shared__ double nn_zero;
     if (tid == 0u) {
         nn_zero = 0.;
     }
-
-    // ---- tensor memory: all 512 columns, 256 per thread (warps w and w + 4 share a quadrant) ----
-    if (warp == 0u) {
-        tm::alloc_all(&tm_base_smem);
-    }
-    tm::fence_before_sync();
 
     // ---- weights: global -> shared through the TMA unit, once per CTA ----
     if (tid == 0u) {
@@ -142,8 +130,6 @@ __global__ void __launch_bounds__(NN_THREADS, 1) k_nn(program P, nn_dev_plan NP,
         }
     }
     nnk::mbar_wait(&wbar, 0u);
-    tm::fence_after_sync();
-    const std::uint32_t tmc = tm_base_smem + (((warp & 3u) * 32u) << 16) + (warp >> 2) * 256u;
 
     const std::uint32_t n_chunks = (D.n + LB - 1u) / LB;
     const bool owner = tid < LB;
@@ -164,6 +150,7 @@ __global__ void __launch_bounds__(NN_THREADS, 1) k_nn(program P, nn_dev_plan NP,
                 const bool hidden = NP.act[L] != 0u;
                 double *zh = hist + NP.hist_off[L];                                  // z: [order][n_out][LB]
                 double *th = zh + static_cast<std::size_t>(p) * n_out * LB;          // activation output
+                double *sh = th + static_cast<std::size_t>(p) * n_out * LB;          // its square
                 // ---- z^[n] = W a^[n] (+ b): one 8 x 8 x k tile per warp and pass ----
                 {
                     const std::uint32_t row_in_tile = lane_id >> 2, kk = lane_id & 3u;
@@ -210,84 +197,53 @@ __global__ void __launch_bounds__(NN_THREADS, 1) k_nn(program P, nn_dev_plan NP,
                 }
                 __syncthreads();
                 if (hidden) {
-                    // ---- tanh and tanh^2, one thread per (neuron, lane); every thread of a warp runs the (warp-wide)
-                    // tensor-memory accesses, the ones without an item on zeros ----
+                    // ---- tanh and tanh^2, one thread per (neuron, lane) ----
                     const std::uint32_t n_items = n_out * LB;
                     const std::size_t so = static_cast<std::size_t>(n_out) * LB; // stride between orders
-                    for (std::uint32_t r = 0; r < NP.tm_ipt; ++r) {
-                        const std::uint32_t it = tid + r * NN_THREADS;
-                        const bool act = it < n_items;
-                        // tanh^2: 48 columns, order i at columns 16 + 2 i (the 16 below order 0 are padding: the eight
-                        // orders below order n are read as ONE aligned window whatever n is).
-                        const std::uint32_t scol = tmc + (NP.tm_slot[L] * NP.tm_ipt + r) * 48u;
-                        const double *zp = zh + (act ? it : 0u);
-                        double *tp = th + (act ? it : 0u);
-                        const double z = act ? zp[n * so] : 0.;
+                    for (std::uint32_t it = tid; it < n_items; it += NN_THREADS) {
+                        const double *zp = zh + it;
+                        double *tp = th + it, *sp = sh + it;
+                        const double z = zp[n * so];
                         double t = 0.;
                         if (n == 0u) {
-                            if (act) {
-                                t = ::tanh(z);
-                            }
+                            t = ::tanh(z);
                         } else {
                             // b^[n] - (1/n) sum_{j=1..n} j (c^[n-j] b^[j]), c = tanh(b)^2 (src/math/tanh.cpp:183-318), j
-                            // ascending: c^[n-j], j = 1..8, is word pair 8 - j of the window that ends below order n
-                            // (j = 9..16: of the window before it). The order is the same for the whole warp: the tests
-                            // on j are uniform branches, nothing is executed for the terms that do not exist. (Threads
-                            // without an item compute on whatever their columns hold; nothing of it is stored.)
+                            // ascending.
                             double acc = 0., jd = 1.;
-                            const double *zq = zp + so;
-                            for (std::uint32_t base = 0; base < n; base += 8u) {
-                                tm::words<16> w;
-                                __syncwarp();
-                                tm::ld(scol + 2u * n - 2u * base, w);
-                                tm::wait_ld(w);
-#pragma unroll
-                                for (int jj = 1; jj <= 8; ++jj) {
-                                    if (base + static_cast<std::uint32_t>(jj) > n) {
-                                        break;
-                                    }
-                                    const double c_i = __hiloint2double(static_cast<int>(w.w[2 * (8 - jj) + 1]),
-                                                                        static_cast<int>(w.w[2 * (8 - jj)]));
-                                    acc = ::fma(jd, c_i * *zq, acc);
-                                    jd += 1.;
-                                    zq += so;
-                                }
+                            const double *zq = zp + so, *cq = sp + (n - 1u) * so;
+                            for (std::uint32_t j = 1; j <= n; ++j) {
+                                acc = ::fma(jd, *cq * *zq, acc);
+                                jd += 1.;
+                                zq += so;
+                                cq -= so;
                             }
                             t = z - acc / static_cast<double>(n);
                         }
-                        if (act) {
-                            tp[n * so] = t;
-                        }
+                        tp[n * so] = t;
                         // Square (src/math/pow.cpp:618-963, exponent 2).
                         double sq = 0.;
-                        if (act) {
-                            if (n == 0u) {
-                                sq = t * t;
+                        if (n == 0u) {
+                            sq = t * t;
+                        } else {
+                            const bool odd = (n & 1u) != 0u;
+                            const std::uint32_t j1 = odd ? (n - 1u) / 2u : (n - 2u) / 2u;
+                            double acc = 0.;
+                            const double *pa = tp + n * so, *pb = tp;
+                            for (std::uint32_t j = 0; j <= j1; ++j) {
+                                acc = ::fma(*pa, *pb, acc);
+                                pa -= so;
+                                pb += so;
+                            }
+                            if (odd) {
+                                sq = acc + acc;
                             } else {
-                                const bool odd = (n & 1u) != 0u;
-                                const std::uint32_t j1 = odd ? (n - 1u) / 2u : (n - 2u) / 2u;
-                                double acc = 0.;
-                                const double *pa = tp + n * so, *pb = tp;
-                                for (std::uint32_t j = 0; j <= j1; ++j) {
-                                    acc = ::fma(*pa, *pb, acc);
-                                    pa -= so;
-                                    pb += so;
-                                }
-                                if (odd) {
-                                    sq = acc + acc;
-                                } else {
-                                    const double h2 = tp[(n / 2u) * so];
-                                    sq = (acc + acc) + h2 * h2;
-                                }
+                                const double h2 = tp[(n / 2u) * so];
+                                sq = (acc + acc) + h2 * h2;
                             }
                         }
-                        tm::words<2> ws;
-                        ws.w[0] = static_cast<std::uint32_t>(__double2loint(sq));
-                        ws.w[1] = static_cast<std::uint32_t>(__double2hiint(sq));
-                        __syncwarp();
-                        tm::st(scol + 16u + n * 2u, ws);
+                        sp[n * so] = sq;
                     }
-                    tm::wait_st();
                     __syncthreads();
                     in = th + static_cast<std::size_t>(n) * n_out * LB;
                 } else {
@@ -416,11 +372,6 @@ __global__ void __launch_bounds__(NN_THREADS, 1) k_nn(program P, nn_dev_plan NP,
             }
         }
         __syncthreads();
-    }
-    tm::fence_before_sync();
-    __syncthreads();
-    if (warp == 0u) {
-        tm::dealloc_all(tm_base_smem);
     }
 }
 

@@ -117,8 +117,7 @@ struct item {
 
 } // namespace
 
-smem_plan make_smem_plan(const hy_program &p, bool fuse, bool fuse_sv, bool spill_private,
-                         std::uint32_t tmem_max_pairs, std::uint32_t tmem_rows)
+smem_plan make_smem_plan(const hy_program &p, bool fuse, bool fuse_sv, bool spill_private)
 {
     smem_plan pl;
     const auto n_eq = p.n_eq, n_uvars = p.n_uvars, order = p.order;
@@ -386,31 +385,6 @@ smem_plan make_smem_plan(const hy_program &p, bool fuse, bool fuse_sv, bool spil
             }
         }
         items.push_back(std::move(it));
-    }
-
-    // ---- tensor-memory residency of the superinstructions' private rows (see smem_plan.hpp) ----
-    {
-        std::uint32_t n_pairs = 0;
-        bool only_fused = !items.empty();
-        for (const auto &it : items) {
-            n_pairs += it.op.opcode == HY_FOP_NBODY_PAIR ? 1u : 0u;
-            // (Sums of single-slot rows become superinstructions further down: checked again at the end.)
-            only_fused = only_fused && (it.op.opcode >= HY_FOP_FIRST || it.op.opcode == HY_OP_SUM);
-        }
-        const bool use_tmem
-            = tmem_max_pairs != 0u && !spill_private && only_fused && n_pairs != 0u && n_pairs <= tmem_max_pairs;
-        pl.tmem = use_tmem ? (tmem_rows >= 3u ? 3u : 2u) : 0u;
-        if (use_tmem) {
-            for (const auto &it : items) {
-                if (it.op.opcode == HY_FOP_NBODY_PAIR) {
-                    dropped[it.defs[3]] = 1; // r^2
-                    dropped[it.defs[4]] = 1; // r^alpha
-                    if (pl.tmem == 3u) {
-                        dropped[it.defs[2]] = 1; // d_2
-                    }
-                }
-            }
-        }
     }
 
     // ---- slot assignment ----
@@ -711,14 +685,6 @@ smem_plan make_smem_plan(const hy_program &p, bool fuse, bool fuse_sv, bool spil
         pl.seg_offsets.push_back(static_cast<std::uint32_t>(pl.ops.size()));
     }
 
-    if (pl.tmem != 0u) {
-        for (const auto &op : pl.ops) {
-            if (op.opcode < HY_FOP_FIRST) {
-                // An elementary op survived: the tensor-memory kernel does not interpret those.
-                return make_smem_plan(p, fuse, fuse_sv, spill_private, 0u, 2u);
-            }
-        }
-    }
     return pl;
 }
 

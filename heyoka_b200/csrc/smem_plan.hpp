@@ -43,9 +43,6 @@ struct smem_plan {
     // resident warps, the rows that only a superinstruction reads (r^2 and r^alpha histories of the pair
     // interaction) are moved out of shared memory (spill_private).
     std::uint32_t n_gslots = 0;
-    // The r^2 / r^alpha histories of the pair interactions live in tensor memory (thread-private, tmem.cuh).
-    // Number of such rows per pair interaction: 0 (none), 2 (r^2, r^alpha) or 3 (+ the third difference d_2).
-    std::uint32_t tmem = 0;
     std::uint32_t n_segments = 0;
     std::uint32_t max_seg_width = 0;
     // Ops in execution order (segment by segment, grouped by opcode inside a segment); operand fields that
@@ -70,12 +67,7 @@ struct smem_plan {
     std::vector<std::uint32_t> svout, svo, sv_cover, sv_parent, sv_phase;
 };
 
-// tmem_max_pairs: if non-zero and the program consists of superinstructions only, with at most that many pair
-// interactions (one per thread of a warp), the r^2 and r^alpha histories of the pair interactions are not given
-// shared-memory rows: the kernel keeps them in tensor memory (smem_plan::tmem is set). tmem_rows = 3 also moves
-// the third coordinate difference of every pair (read only by the pair's own thread as well).
-smem_plan make_smem_plan(const hy_program &, bool fuse = true, bool fuse_sv = true, bool spill_private = false,
-                         std::uint32_t tmem_max_pairs = 0, std::uint32_t tmem_rows = 2);
+smem_plan make_smem_plan(const hy_program &, bool fuse = true, bool fuse_sv = true, bool spill_private = false);
 
 } // namespace heyoka_b200::detail
 

@@ -1,4 +1,4 @@
-/* heyoka_b200 — C ABI of the B200-native batch Taylor integrator.
+/* heyoka_b200 — C ABI of the H100-native batch Taylor integrator.
  *
  * This is the drop-in boundary for heyoka's taylor_adaptive_batch<double> hot path
  * (bluescarni/heyoka @ 9c91f71). The reference funnels every step through three JIT-compiled C
@@ -14,7 +14,7 @@
  * in the reference (double-length time update, finiteness scan, outcome; src/taylor_adaptive_batch.cpp:702-727)
  * and the whole propagate_until() loop (:1372-1527) run inside the kernels, (iii) instead of LLVM IR
  * the Taylor decomposition is lowered to a flat opcode program (hy_program) interpreted by
- * hand-written sm_100a kernels. No LLVM, no JIT, no CPU fallback: every compute entry point fails
+ * hand-written sm_90a kernels. No LLVM, no JIT, no CPU fallback: every compute entry point fails
  * with HY_ERR_CUDA if no CUDA device is usable.
  *
  * All functions return HY_OK (0) or a negative error code; hy_last_error() returns a thread-local
@@ -379,12 +379,11 @@ int hy_batch_set_launch_config(hy_batch *, uint32_t block_threads, uint32_t bloc
 
 /* Kernel selection. tape_mode: 0 = automatic (shared-memory tape when the system's tape fits in an SM's shared
  * memory, else mode 4), 1 = force the one-thread-per-lane HBM-tape kernel, 2 = force the shared-memory kernel (error if it
- * does not fit), 3 = idem, but never keep rows in tensor memory, 4 = the same warp-cooperative kernel with the
+ * does not fit), 3 = the same as 2 (kept for compatibility), 4 = the same warp-cooperative kernel with the
  * tape in global memory, 5 = idem with a whole CTA (instead of a warp) working on a chunk of lanes; the automatic
  * mode picks 4 or 5 when shared memory is too small; 6 / 7 = the dedicated N-body kernel (warp / CTA teams; error if
  * the program is not N-body-shaped, see csrc/nb_plan.hpp), which the automatic mode prefers whenever the program
- * qualifies (lanes_per_thread then selects the storage of the private history rows: 0 automatic, 1 tensor memory,
- * 2 shared memory only; lanes_per_warp = lanes per team); 8 = the dense-network kernel; 9 = the N-body kernel with one
+ * qualifies (lanes_per_thread is ignored; lanes_per_warp = lanes per team); 8 = the dense-network kernel; 9 = the N-body kernel with one
  * thread per lane (programs with ONE pair interaction, e.g. the two-body problem; the automatic mode takes it when it
  * applies, HEYOKA_B200_NB_LANE=0 turns that off). lanes_per_warp (1..32, power of two) / lanes_per_thread (1, 2 or 4, dividing lanes_per_warp)
  * only apply to the shared-memory kernel; 0 = automatic. block_threads = 32 x warps per block.
@@ -399,7 +398,7 @@ typedef struct hy_kernel_info {
     uint32_t n_segments;          /* dependency levels of the decomposition (cf. src/taylor_02.cpp:105-207) */
     uint32_t n_fused;             /* superinstructions found by the planner (fused N-body pair interactions) */
     uint32_t n_sms;
-    uint32_t tmem_cols_per_warp;  /* tensor-memory columns per warp (0: tensor memory unused) */
+    uint32_t tmem_cols_per_warp;  /* always 0: sm_90 has no tensor memory (field kept for ABI compatibility) */
     uint32_t reserved;
 } hy_kernel_info;
 int hy_batch_get_kernel(const hy_batch *, hy_kernel_info *out);

@@ -1,4 +1,4 @@
-// heyoka_b200 — taylor_adaptive_batch<double>: the reference's batch integrator class, backed by the B200
+// heyoka_b200 — taylor_adaptive_batch<double>: the reference's batch integrator class, backed by the H100
 // kernels through the C ABI (include/heyoka_b200.h).
 //
 // Mirrors include/heyoka/taylor.hpp:780-1121 (bluescarni/heyoka @ 9c91f71) for T = double: same constructor

@@ -134,7 +134,8 @@ int main()
             REQUIRE(std::abs(by_ptr[1] - (0.1 * std::cos(1.5) + 1.1 * std::sin(1.5))) < 1e-13);
             // get_times() / get_tcs() (include/heyoka/continuous_output.hpp:198-199): (n_steps + 2) rows of times (start,
             // the end of every iteration, the padding), [n_steps][dim][order + 1][batch] Taylor coefficients; at the
-            // start of an iteration the output is the order-0 coefficients of that iteration.
+            // start of an iteration the output is the order-0 coefficients of that iteration (up to the low part of the
+            // double-length start time: tms holds the high parts).
             const auto n_steps = co->get_n_steps();
             const auto &tms = co->get_times();
             const auto &tcs = co->get_tcs();
@@ -147,7 +148,8 @@ int main()
                 const auto out = (*co)(tms.data() + k * 4u);
                 for (std::size_t var = 0; var < 2u; ++var) {
                     for (std::size_t i = 0; i < 4u; ++i) {
-                        REQUIRE(out[var * 4u + i] == tcs[((k * 2u + var) * ord1) * 4u + i]);
+                        REQUIRE(std::abs(out[var * 4u + i] - tcs[((k * 2u + var) * ord1) * 4u + i])
+                                < 1e-15 * std::max(1., std::abs(tms[k * 4u + i])));
                     }
                 }
             }

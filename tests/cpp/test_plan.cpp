@@ -29,18 +29,12 @@ int main()
     REQUIRE(P.n_uvars == 234u);
 
     // Reference tape: n_uvars * order + n_eq (src/taylor_02.cpp:1227-1233) = 234 * 20 + 36 = 4716 doubles per lane.
-    const auto plain = detail::make_smem_plan(P, false, false, false, 0);
-    const auto fused = detail::make_smem_plan(P, true, true, false, 0);
-    const auto tm2 = detail::make_smem_plan(P, true, true, false, 32, 2);
-    const auto tm3 = detail::make_smem_plan(P, true, true, false, 32, 3);
-    std::printf("slots per lane: unfused %u, fused %u, tmem2 %u, tmem3 %u\n", plain.n_slots, fused.n_slots, tm2.n_slots,
-                tm3.n_slots);
+    const auto plain = detail::make_smem_plan(P, false, false, false);
+    const auto fused = detail::make_smem_plan(P, true, true, false);
+    std::printf("slots per lane: unfused %u, fused %u\n", plain.n_slots, fused.n_slots);
     REQUIRE(plain.n_slots < 234u * 21u / 2u);
     REQUIRE(fused.n_fused == 15u && fused.n_segments == 2u);
     REQUIRE(fused.n_slots == 1761u);            // 16 warps x 2 lanes would need 2 x 8 x 1761 x 16 = 450 KB: 8 warps fit
-    REQUIRE(tm2.tmem == 2u && tm2.n_slots == 1761u - 2u * 15u * 21u);
-    REQUIRE(tm3.tmem == 3u && tm3.n_slots == 1761u - 3u * 15u * 21u); // 816: 16 warps x 2 lanes in 209 KB
-    REQUIRE(detail::make_smem_plan(P, true, true, false, 8, 2).tmem == 0u); // more pairs than threads allowed
     // Level 0 = the 15 pair interactions, level 1 = the 18 sums.
     REQUIRE(fused.seg_offsets.size() == 3u && fused.seg_offsets[1] - fused.seg_offsets[0] == 15u
             && fused.seg_offsets[2] - fused.seg_offsets[1] == 18u);
@@ -59,18 +53,17 @@ int main()
             REQUIRE(banks.size() == 8u);
         }
     }
-    // model::nbody with 32 bodies: 496 pair interactions in level 0 (too many for the one-pair-per-thread tensor-memory
-    // layout), sums of up to 31 terms split at 8 (src/taylor_01.cpp split_sums), a tape far beyond shared memory.
+    // model::nbody with 32 bodies: 496 pair interactions in level 0, sums of up to 31 terms split at 8 (src/taylor_01.cpp split_sums), a tape far beyond shared memory.
     {
         std::vector<double> m32(32, 1e-4);
         m32[0] = 1.;
         auto sys32 = model::nbody(32, kw::masses = m32);
         auto [dc32, sv32] = taylor_decompose_sys(sys32, {});
         const auto P32 = detail::lower_decomposition(dc32, 192, 0, 20, false);
-        const auto pl = detail::make_smem_plan(P32, true, true, false, 32, 3);
+        const auto pl = detail::make_smem_plan(P32, true, true, false);
         std::printf("N = 32: %u u variables, %u superinstructions, %u levels, %u slots per lane\n", P32.n_uvars,
                     pl.n_fused, pl.n_segments, pl.n_slots);
-        REQUIRE(pl.n_fused == 496u && pl.tmem == 0u);
+        REQUIRE(pl.n_fused == 496u);
         REQUIRE(pl.seg_offsets[1] - pl.seg_offsets[0] == 496u);
         REQUIRE(pl.n_slots * 8u > 227u * 1024u); // one lane alone does not fit in an SM's shared memory
     }

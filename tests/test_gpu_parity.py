@@ -24,19 +24,20 @@ KERNELS = {
     "hbm": dict(tape="hbm"),
     "global": dict(tape="global"),  # the cooperative kernel with the tape in global memory
     "global-cta": dict(tape="global-cta"),  # idem, a whole CTA per chunk of lanes
-    "smem-auto": dict(tape="smem"),  # tensor memory for the pair interactions where it applies
-    "smem-notmem": dict(tape="smem-notmem"),
+    "smem-auto": dict(tape="smem"),
+    "smem-notmem": dict(tape="smem-notmem"),  # (the same kernel as "smem": the API keeps the name)
     "smem-L8N2": dict(tape="smem", lanes_per_warp=8, lanes_per_thread=2),
     "smem-L2N1": dict(tape="smem", lanes_per_warp=2, lanes_per_thread=1, block_threads=64),
-    "smem-L2N2": dict(tape="smem", lanes_per_warp=2, lanes_per_thread=2),  # two rows per pair in tensor memory
+    "smem-L2N2": dict(tape="smem", lanes_per_warp=2, lanes_per_thread=2),
     "smem-L4N4": dict(tape="smem", lanes_per_warp=4, lanes_per_thread=4, block_threads=32),
-    # The dedicated N-body kernel (nb_kernel.cuh; N-body-shaped programs only, the other tests skip): private rows in
-    # tensor memory / in shared memory only / 12 warps per CTA (168 registers per thread).
+    # The dedicated N-body kernel (nb_kernel.cuh; N-body-shaped programs only, on the others the tests check that it is
+    # refused, see _refused()): default / with lanes_per_thread given (ignored) / 12 warps per CTA (168 registers per
+    # thread) / one lane per team.
     "nbody": dict(tape="nbody"),
     "nbody-smem": dict(tape="nbody", lanes_per_thread=2),
     "nbody-384": dict(tape="nbody", lanes_per_thread=1, block_threads=384),
     "nbody-L1": dict(tape="nbody", lanes_per_warp=1, block_threads=128),
-    # One thread per lane (nb1_kernel.cuh; programs with ONE pair interaction only): tensor memory / shared memory only.
+    # One thread per lane (nb1_kernel.cuh; programs with ONE pair interaction only): default / lanes_per_thread given.
     "nbody-lane": dict(tape="nbody-lane"),
     "nbody-lane-smem": dict(tape="nbody-lane", lanes_per_thread=2),
 }
@@ -45,6 +46,23 @@ KERNELS = {
 @pytest.fixture(params=list(KERNELS), scope="module")
 def kernel(request):
     return KERNELS[request.param]
+
+
+def _refused(kernel, sys, **program_kw):
+    """The dedicated N-body kernels run N-body-shaped programs only (nb_plan.hpp; the one-thread-per-lane form: one pair
+    interaction). Forcing one of them on another program must fail with the documented error, never fall back to another
+    kernel: for those (kernel, program) combinations that refusal is what the test checks, and it returns True. False:
+    the kernel runs the program (and the test goes on with it)."""
+    if not kernel["tape"].startswith("nbody"):
+        return False
+    b = hb.Batch(hb.Program(sys, **program_kw), 1)
+    try:
+        b.set_kernel(**kernel)
+    except ValueError as e:
+        assert "The N-body kernel cannot run this program" in str(e), str(e)
+        return True
+    assert b.kernel_info()["tape"] == kernel["tape"]
+    return False
 
 
 def rel_err(a, b, floor=1e-6):
@@ -72,6 +90,8 @@ def tc_err(tc_a, tc_b, h):
 
 def test_tutorial_batch_mode_gpu(kernel):
     """doc/tut_batch_mode.rst end to end on the GPU (same fixture that pins the oracle)."""
+    if _refused(kernel, sys_tutorial()):
+        return
     g = golden("tut_batch_mode.json")
     ta = hb.taylor_adaptive_batch(sys_tutorial(), [g["x0"], g["v0"]], 4, pars=[g["alpha"]], kernel=kernel)
     assert ta.get_order() == 20
@@ -107,6 +127,8 @@ def test_tutorial_batch_mode_gpu(kernel):
 
 
 def _step_parity(kernel, sys, state, batch, pars=None, time=0.0, ha=False, n_steps=3, tol=1e-13, max_delta_t=None):
+    if _refused(kernel, sys, high_accuracy=ha):
+        return
     P = hb.Program(sys, high_accuracy=ha)
     o = oracle.OracleIntegrator(P, state, batch, pars=pars, time=time, mode=oracle.FMA)
     ta = hb.taylor_adaptive_batch(sys, state, batch, pars=pars, time=time, high_accuracy=ha, kernel=kernel)
@@ -164,6 +186,8 @@ def test_step_parity_outer_ss(kernel, ha, batch):
 
 
 def test_step_backward_and_limits(kernel):
+    if _refused(kernel, sys_outer_ss()):
+        return
     st = outer_ss_batch_state(8)
     P = hb.Program(sys_outer_ss())
     o = oracle.OracleIntegrator(P, st, 8, mode=oracle.FMA)
@@ -183,6 +207,8 @@ def test_step_backward_and_limits(kernel):
 @pytest.mark.parametrize("ha", [False, True])
 def test_propagate_parity_outer_ss(kernel, ha):
     """100 years of the perturbed outer Solar System: identical step counts, final state to 1e-12."""
+    if _refused(kernel, sys_outer_ss(), high_accuracy=ha):
+        return
     batch = 40
     st = outer_ss_batch_state(batch)
     P = hb.Program(sys_outer_ss(), high_accuracy=ha)
@@ -223,6 +249,8 @@ def test_propagate_parity_reference_default_mode(mode):
 
 def test_propagate_exact_step_counts_gpu(kernel):
     """test/taylor_adaptive_batch.cpp:586-598 on the GPU."""
+    if _refused(kernel, sys_pendulum()):
+        return
     ta = hb.taylor_adaptive_batch(sys_pendulum(), [[0.05, 0.06], [0.025, 0.026]], 2, kernel=kernel)
     ta2 = hb.taylor_adaptive_batch(sys_pendulum(), [[0.05, 0.06], [0.025, 0.026]], 2, kernel=kernel)
     ta.propagate_until([10., 11.], max_delta_t=[1e-4, 5e-5])
@@ -238,6 +266,8 @@ def test_propagate_exact_step_counts_gpu(kernel):
 
 
 def test_propagate_per_lane_times_and_dfloat(kernel):
+    if _refused(kernel, sys_pendulum()):
+        return
     batch = 35
     rng = np.random.default_rng(5)
     st = np.stack([rng.uniform(-1, 1, batch), rng.uniform(-1, 1, batch)])
@@ -259,6 +289,8 @@ def test_global_exits_match_reference_semantics(kernel):
     """max_steps counts iterations and turns EVERY outcome into step_limit; a non-finite lane stops EVERY
     lane at that iteration (src/taylor_adaptive_batch.cpp:1462-1467, :1516-1526). Checked against the
     oracle's lock-step loop."""
+    if _refused(kernel, sys_outer_ss()):
+        return
     batch = 6
     st = outer_ss_batch_state(batch)
     P = hb.Program(sys_outer_ss())
@@ -291,6 +323,8 @@ def test_global_exits_match_reference_semantics(kernel):
 
 
 def test_dense_output(kernel):
+    if _refused(kernel, sys_outer_ss(), high_accuracy=True):
+        return
     batch = 9
     st = outer_ss_batch_state(batch)
     P = hb.Program(sys_outer_ss(), high_accuracy=True)
@@ -316,6 +350,8 @@ def test_propagate_early_lanes_last_h_and_tc(kernel):
     loop (src/taylor_adaptive_batch.cpp:1372-1397): on return last_h = 0 and, with write_tc, the Taylor coefficients
     are re-expanded about the final state. The device-resident loop reproduces both (one masked zero-length step);
     compared against the oracle's lock-step loop, then through update_d_output()."""
+    if _refused(kernel, sys_outer_ss(), high_accuracy=True):
+        return
     batch = 10
     st = outer_ss_batch_state(batch)
     tf = np.linspace(2.0, 11.0, batch)  # different numbers of steps per lane
@@ -416,10 +452,10 @@ def test_kernel_selection_info():
     CTA teams for 32 bodies), the shared-memory tape otherwise; every strategy can be forced."""
     b = hb.Batch(hb.Program(sys_outer_ss(), high_accuracy=True), 64)
     ki = b.kernel_info()
-    # 15 pair interactions x 2 lanes, one per thread; r^2, d_z, r^-3 live in tensor memory as (even, odd) order pairs:
-    # 10 pairs x 12 columns; 12 warps of 2 lanes per SM (168 registers per thread: no spills in the pair interaction).
-    assert ki["tape"] == "nbody" and ki["lanes_per_warp"] == 2 and ki["tmem_cols_per_warp"] == 120
-    assert ki["block_threads"] == 384 and ki["smem_bytes"] <= 227 * 1024
+    # 15 pair interactions x 2 lanes, one per thread, every private row in shared memory: 7 warps of 2 lanes fit in the
+    # 227 KB of an H100 SM.
+    assert ki["tape"] == "nbody" and ki["lanes_per_warp"] == 2 and ki["tmem_cols_per_warp"] == 0
+    assert ki["block_threads"] == 224 and ki["smem_bytes"] <= 227 * 1024
     b.set_kernel("nbody", lanes_per_thread=2)
     ki = b.kernel_info()
     assert ki["tape"] == "nbody" and ki["tmem_cols_per_warp"] == 0
@@ -427,11 +463,11 @@ def test_kernel_selection_info():
     ki = b.kernel_info()
     assert ki["tape"] == "smem" and ki["tape_slots_per_lane"] < 234 * 21 / 2
     assert ki["smem_bytes"] <= 227 * 1024
-    # The generic cooperative kernel: 3 rows x 21 orders x 2 words per pair interaction in tensor memory.
-    assert ki["tmem_cols_per_warp"] == 126 and ki["block_threads"] == 512 and ki["lanes_per_thread"] == 1
+    # The generic cooperative kernel: 8 warps of 2 lanes, two per thread, in shared memory.
+    assert ki["tmem_cols_per_warp"] == 0 and ki["block_threads"] == 256 and ki["lanes_per_thread"] == 2
     b.set_kernel("smem", lanes_per_warp=2, lanes_per_thread=2)
     ki = b.kernel_info()
-    assert ki["tmem_cols_per_warp"] == 168 and ki["block_threads"] == 384
+    assert ki["tmem_cols_per_warp"] == 0 and ki["block_threads"] == 256
     b.set_kernel("smem-notmem")
     ki = b.kernel_info()
     assert ki["tmem_cols_per_warp"] == 0 and ki["block_threads"] == 256
@@ -466,6 +502,8 @@ def test_closed_form_jets_gpu(case, gold, kernel):
     one step with write_tc, jets against the symbolic closed forms to the reference's tolerance."""
     from closed_form_cases import EPS_MUL, ORDER, TOL, batch_of, hb_system
     from test_oracle_golden import approximately
+    if _refused(kernel, hb_system(hb, case), tol=TOL):
+        return
     BATCH = batch_of(case)
     ta = hb.taylor_adaptive_batch(hb_system(hb, case), np.array(gold["state"], dtype=float).reshape(2, BATCH), BATCH,
                                   time=gold["time"] if gold["time"] else 0.0, tol=TOL, kernel=kernel)
@@ -481,6 +519,8 @@ def test_propagate_grid_oscillator_gpu(kernel):
     """test/taylor_adaptive_batch.cpp:269-385: regular and random grids, forward and backward, against the closed
     form (the reference's tolerances) and against the oracle's restatement (step counts, outcomes, values)."""
     from test_oracle_golden import OSC_STATE, approximately, grid_fixtures, sys_oscillator
+    if _refused(kernel, sys_oscillator()):
+        return
     for name, grid, tol in grid_fixtures():
         ta = hb.taylor_adaptive_batch(sys_oscillator(), OSC_STATE, 4, kernel=kernel)
         ret = ta.propagate_grid(grid)
@@ -548,6 +588,8 @@ def test_propagate_grid_errors_and_trivial_cases():
 @pytest.mark.gpu
 def test_propagate_grid_limits_match_oracle(kernel):
     """max_delta_t and max_steps (early exit: remaining rows NaN, every outcome step_limit), 6-body system."""
+    if _refused(kernel, sys_outer_ss(), high_accuracy=True):
+        return
     st = outer_ss_batch_state(5, perturb=1e-3, seed=3)
     grid = np.linspace(0.0, 4.0, 41)[:, None] * np.array([1.0, 1.1, 0.9, 1.05, 0.95])[None, :]
     for kw in (dict(max_delta_t=[0.05, 0.2, 0.3, 0.11, 1.0]), dict(max_steps=5), dict()):
@@ -632,6 +674,8 @@ def test_continuous_output_gpu(kernel):
     propagation of the same integrator (100 eps), the closed form, and the oracle's restatement (same number of
     recorded iterations, same values)."""
     from test_oracle_golden import approximately, cout_fixture, sys_oscillator
+    if _refused(kernel, sys_oscillator()):
+        return
     ic, final_tm, grid = cout_fixture()
     for ha in (False, True):
         ta = hb.taylor_adaptive_batch(sys_oscillator(), ic, 4, high_accuracy=ha, kernel=kernel)
@@ -692,6 +736,8 @@ def test_two_body_kepler_conservation_gpu(kernel):
     step agrees with a one-lane integrator taking the same step, and the Keplerian elements of both bodies are
     conserved to 1e4 epsilon."""
     from common import check_kepler_conservation, sys_two_body_symmetric, two_body_kepler_fixture
+    if _refused(kernel, sys_two_body_symmetric()):
+        return
     from test_oracle_golden import approximately
     kep, st = two_body_kepler_fixture()
     ta = hb.taylor_adaptive_batch(sys_two_body_symmetric(), st, 4, kernel=kernel)

@@ -1,4 +1,4 @@
-// FP64 roofline microbenchmarks for sm_100a (B200): the denominators of every "fraction of FP64 peak" in this repo.
+// FP64 roofline microbenchmarks for sm_90a (H100): the denominators of every "fraction of FP64 peak" in this repo.
 //
 //   dfma_tput   dependent-free DFMA streams (8 chains per thread, full occupancy)  -> TFLOP/s (2 flop per FMA)
 //   dadd_tput   idem with DADD (1 flop each)
@@ -6,7 +6,7 @@
 //   dmma_tput   mma.sync.aligned.m8n8k4.f64 streams (4 accumulator tiles per warp) -> TFLOP/s (2*8*8*4 flop each)
 //   dmma_lat    one dependent DMMA chain in one warp                               -> cycles per DMMA
 //
-// Build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o tools/bin/fp64_peak tools/fp64_peak.cu
+// Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o tools/bin/fp64_peak tools/fp64_peak.cu
 // Run (GPU box): tools/bin/fp64_peak > gpurun_out/fp64_peak.json
 #include <cstdio>
 #include <cstdlib>
