@@ -39,3 +39,23 @@ nb_family HY_NB_CAT(nb_family_lt, HY_NB_LT, _cta, HY_NB_CTA)()
 }
 
 } // namespace heyoka_b200::detail
+
+#if defined(HY_NB_PHASE_CLOCK)
+// The phase counters of this family's kernels (nb_kernel.cuh): copies the first n / NB_PH_SLOTS teams' counters to out
+// and resets them all; with out == nullptr only resets them. Returns the number of teams the counters have room for,
+// or -1 on a CUDA error.
+extern "C" int HY_NB_CAT(hy_nb_phase_clock_lt, HY_NB_LT, _cta, HY_NB_CTA)(unsigned long long *out, std::size_t n)
+{
+    namespace hd = heyoka_b200::dev;
+    constexpr std::size_t total = static_cast<std::size_t>(hd::nb_phase_teams) * hd::NB_PH_SLOTS;
+    n = n < total ? n : total;
+    if (out != nullptr && cudaMemcpyFromSymbol(out, hd::nb_phase_cycles, n * sizeof(unsigned long long)) != cudaSuccess) {
+        return -1;
+    }
+    static const unsigned long long zero[total] = {};
+    if (cudaMemcpyToSymbol(hd::nb_phase_cycles, zero, sizeof(zero)) != cudaSuccess) {
+        return -1;
+    }
+    return static_cast<int>(hd::nb_phase_teams);
+}
+#endif

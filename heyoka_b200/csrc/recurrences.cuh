@@ -659,15 +659,22 @@ __device__ __forceinline__ double std_min(double a, double b)
 
 // taylor_determine_h() (src/taylor_00.cpp:102-273) from the three infinity norms: Jorba-Zou step size,
 // clamped to |max_delta_t|, signed like max_delta_t.
-__device__ __forceinline__ double h_from_norms(const program &P, double m0, double mp, double mp1, double max_delta_t)
+// (The program's three constants as values: for out-of-line callers, which would otherwise copy the program to
+// local memory to pass it by reference.)
+__device__ __forceinline__ double h_from_norms(double inv_p, double inv_pm1, double rhofac, double m0, double mp,
+                                               double mp1, double max_delta_t)
 {
     const double num_rho = (m0 <= 1.) ? 1. : m0;
-    const double rho_o = ::pow(num_rho / mp, P.inv_p);
-    const double rho_om1 = ::pow(num_rho / mp1, P.inv_pm1);
+    const double rho_o = ::pow(num_rho / mp, inv_p);
+    const double rho_om1 = ::pow(num_rho / mp1, inv_pm1);
     const double rho_m = std_min(rho_o, rho_om1);
-    double h = rho_m * P.rhofac;
+    double h = rho_m * rhofac;
     h = std_min(h, fabs(max_delta_t));
     return (max_delta_t < 0.) ? -h : h;
+}
+__device__ __forceinline__ double h_from_norms(const program &P, double m0, double mp, double mp1, double max_delta_t)
+{
+    return h_from_norms(P.inv_p, P.inv_pm1, P.rhofac, m0, mp, mp1, max_delta_t);
 }
 
 // Evaluation of one Taylor polynomial at h: Horner (src/taylor_00.cpp:279-351) or compensated summation of
