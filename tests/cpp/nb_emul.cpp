@@ -219,6 +219,23 @@ int nb_emul_plan(const hy_program *p, std::uint32_t *out, char *why, std::size_t
     return static_cast<int>(pl.why.size());
 }
 
+// Sizes that setup_nb() (batch.cu) lays out shared memory with, for a team of `tt` threads owning `lt` lanes, `nl` per
+// thread in the summation phase: out[0] = rounds of the role table, out[1] = its records, out[2] = constants,
+// out[3] = row stride of the fac table. Returns 0, -1 if the program does not qualify.
+int nb_emul_roles(const hy_program *p, std::uint32_t tt, std::uint32_t lt, std::uint32_t nl, std::uint32_t *out)
+{
+    const auto pl = hb::detail::make_nb_plan(*p);
+    if (!pl.ok) {
+        return -1;
+    }
+    const auto roles = hb::detail::make_nb_roles(pl, tt, lt, nl);
+    out[0] = roles.n_rounds;
+    out[1] = static_cast<std::uint32_t>(roles.table.size());
+    out[2] = static_cast<std::uint32_t>(pl.consts.size());
+    out[3] = pl.fac_stride;
+    return 0;
+}
+
 // Jets of the `lt` lanes of ONE team of `tt` threads. state[n_eq][lt] -> coef[lt][n_eq][order + 1] (state variables),
 // and, per pair interaction i and lane l: u_idx[i * 8 + {0..2: d_k, 3: r2, 4: q, 5..7: m_k}] = u variable index,
 // u_rows[((i * lt + l) * 8 + r) * n_ord + o] = coefficient of order o (n_ord = 2 * ceil(order / 2)).

@@ -74,14 +74,98 @@ def test_plan_shapes():
         assert info[0] == 0 and why != "", (info, why)
 
 
+# ---- the systems x orders x team shapes that tests/test_gpu_nbody_shapes.py runs on the device ----
+# name -> (bodies, masses, pair interactions). The comments give the automatic shape of the device kernel. (Planets of
+# unequal masses: with unit masses the right-hand side simplifies to negations the planner does not take for pair
+# outputs, and the program runs on the generic kernel instead.)
+_PLANETS = [1.] + [1e-3 * (b + 1) for b in range(1, 12)]
+NB_SYSTEMS = {
+    "nbody3_m1": (3, [1.], 2),                  # LT 16: one massive body, the massless-massless pair is dropped
+    "nbody3": (3, [1., 0.5, 0.2], 3),           # LT 8
+    "nbody4": (4, _PLANETS[:4], 6),            # LT 4
+    "nbody4_m0102": (4, [0., 1., 0., 2.], 5),   # LT 4, massless bodies first
+    "nbody5_m1_01": (5, [1., 0.1], 7),          # LT 4, three massless bodies at the end
+    "nbody5": (5, _PLANETS[:5], 10),           # LT 2
+    "nbody8": (8, _PLANETS[:8], 28),           # LT 1, 4 idle threads per warp
+    "nbody9": (9, _PLANETS[:9], 36),           # CTA teams: the first count above a warp
+    "nbody12": (12, _PLANETS[:12], 66),        # CTA teams, two summation levels
+    "two_body_m10": (2, [1., 0.], 1),           # k_nb1: the second body's accelerations are the number 0
+    "two_body_m104": (2, [1., 0.4], 1),         # k_nb1: both bodies pull (rescaled pair outputs)
+}
+
+
+def nb_order_tol(order):
+    """The tolerance of a given Taylor order: 0 (the default, order 20) for order 20, else exp(-2 (order - 1))
+    (order = ceil(1 - ln(tol) / 2), src/taylor_00.cpp), nudged up by 0.1 % so that the rounding of the logarithm cannot
+    change the order."""
+    return 0. if order == 20 else float(np.exp(-2. * (order - 1)) * 1.001)
+
+
+def nb_system(name):
+    n, masses, _ = NB_SYSTEMS[name]
+    return hb.model.nbody(n, masses=masses)
+
+
+def nb_order_program(name, order):
+    """The program of system `name` at the given Taylor order."""
+    tol = nb_order_tol(order)
+    P = hb.Program(nb_system(name)) if tol == 0. else hb.Program(nb_system(name), tol=tol)
+    assert P.order == order, (name, order, P.order)
+    return P
+
+
+def nb_lane_states(name, batch, seed=0):
+    """[6 n, batch] states of system `name` whose lanes differ by O(1): body b (b >= 1) on a near-circular orbit of
+    radius 1.5 b + U(0, 0.5) with a random phase per lane and body, speeds 0.97-1.03 times the circular one about the
+    mass inside it, small inclinations; body 0 near the origin. Bodies of a lane start at least 1 apart, so that no
+    close approach shrinks the steps of a short propagation. A lane mix-up in a kernel then moves its results by O(1), not by a perturbation."""
+    n, masses, _ = NB_SYSTEMS[name]
+    masses = list(masses) + [0.] * (n - len(masses))
+    rng = np.random.default_rng(seed)
+    st = np.zeros((6 * n, batch))
+    st[0:3] = 0.05 * rng.uniform(-1., 1., (3, batch))
+    st[3:6] = 0.05 * rng.uniform(-1., 1., (3, batch))
+    for b in range(1, n):
+        r = 1.5 * b + rng.uniform(0., 0.5, batch)
+        ph = rng.uniform(0., 2. * np.pi, batch)
+        v = np.sqrt(max(sum(masses[:b]), 0.5) / r) * rng.uniform(0.97, 1.03, batch)
+        st[6 * b + 0], st[6 * b + 1], st[6 * b + 2] = r * np.cos(ph), r * np.sin(ph), rng.uniform(-0.1, 0.1, batch)
+        st[6 * b + 3], st[6 * b + 4], st[6 * b + 5] = -v * np.sin(ph), v * np.cos(ph), rng.uniform(-0.05, 0.05, batch)
+    return st
+
+
+def nb_team_shapes(n_pairs):
+    """(threads per team, lanes per team) of every team shape the device kernel has: a warp with each power-of-two
+    number of lanes whose pairs fit in its 32 threads, and a CTA of 512 threads with one lane."""
+    return [(32, lt) for lt in (1, 2, 4, 8, 16, 32) if lt * n_pairs <= 32] + [(512, 1)]
+
+
+NB_ORDERS = (20, 15, 5, 25)                   # default, odd, low (warp teams of 512 threads, CTA rows on chip), high
+NB_ORDERS_EXTRA = {"nbody3": (36, 71), "two_body_m10": (2, 3, 4, 71), "two_body_m104": (3, 4, 36)}
+
+
+def _sweep_cases():
+    out = []
+    for name, (_, _, n_pairs) in NB_SYSTEMS.items():
+        for order in NB_ORDERS + NB_ORDERS_EXTRA.get(name, ()):
+            out += [("%s@%d" % (name, order), tt, lt) for tt, lt in nb_team_shapes(n_pairs)]
+    return out
+
+
 @pytest.mark.parametrize("name,tt,lt", [("outer_ss", 32, 2), ("outer_ss", 32, 1), ("two_body", 32, 32), ("two_body", 32, 4),
-                                        ("nbody32", 512, 1), ("outer_ss_odd_order", 32, 2)])
+                                        ("nbody32", 512, 1), ("outer_ss_odd_order", 32, 2)] + _sweep_cases())
 def test_two_order_blocks_match_oracle(name, tt, lt):
     """Every coefficient the blocked evaluation produces (coordinate differences, r^2, r^alpha, products, state
     variables) equals the oracle's sequential+FMA jet bit for bit, for the team shapes the kernel uses (threads per
-    team, lanes per team): the pair threads, the output-slot layout and the per-thread role table of the sums."""
+    team, lanes per team): the pair threads, the output-slot layout and the per-thread role table of the sums.
+    "system@order": the systems and orders of tests/test_gpu_nbody_shapes.py, so that a failure there can be put on the
+    device code."""
     lib = _emul()
-    if name == "outer_ss":
+    if "@" in name:
+        sys_name, order = name.split("@")
+        P = nb_order_program(sys_name, int(order))
+        st = nb_lane_states(sys_name, lt, seed=lt)
+    elif name == "outer_ss":
         P, st = hb.Program(sys_outer_ss(), high_accuracy=True), outer_ss_batch_state(lt)
     elif name == "outer_ss_odd_order":
         P, st = hb.Program(sys_outer_ss(), tol=1e-12), outer_ss_batch_state(lt)
@@ -92,6 +176,8 @@ def test_two_order_blocks_match_oracle(name, tt, lt):
         P, st = hb.Program(sys_nbody32()), nbody32_batch_state(lt)
     info, why = _plan(lib, P)
     assert info[0] == 1, why
+    if "@" in name:
+        assert info[1] == NB_SYSTEMS[sys_name][2], info
     coef, u_idx, u_rows = _emul_jet(lib, P, st, info[1], tt, lt)
     for lane in range(lt):
         tape = oracle.jet(P, st, lane=lane, mode=oracle.FMA)  # [order + 1, n_uvars]; u variables: orders < order
