@@ -15,6 +15,7 @@
 
 #include "nb_core.hpp"
 #include "nb_plan.hpp"
+#include "smem_plan.hpp"
 
 namespace hb = heyoka_b200;
 using hb::nb::d2;
@@ -233,6 +234,37 @@ int nb_emul_roles(const hy_program *p, std::uint32_t tt, std::uint32_t lt, std::
     out[1] = static_cast<std::uint32_t>(roles.table.size());
     out[2] = static_cast<std::uint32_t>(pl.consts.size());
     out[3] = pl.fac_stride;
+    return 0;
+}
+
+// The cooperative plan (make_smem_plan(), smem_plan.hpp) that hy_batch builds with the given options: out[0] = n_slots,
+// out[1] = n_gslots, out[2] = work items, out[3] = segments, out[4] = 1 if an item is an elementary op (kernel mode 1)
+// and 0 if all are superinstructions (mode 0), out[5] = bytes of the table blob, restating make_plan_blob() (batch.cu)
+// word by word.
+int coop_emul_plan(const hy_program *p, int fuse, int fuse_sv, int spill, std::uint32_t *out)
+{
+    const auto pl = hb::detail::make_smem_plan(*p, fuse != 0, fuse_sv != 0, spill != 0);
+    std::size_t w = 20u; // dev::coop_header
+    const auto align = [&](std::size_t a) { w = (w + a - 1u) / a * a; };
+    align(4);
+    w += 8u * pl.ops.size() + pl.seg_offsets.size() + pl.args.size() + pl.aux.size();
+    align(2);
+    w += 2u * (p->consts.size() + pl.extra_consts.size());
+    align(2);
+    w += 2u * (p->order + 3u); // reciprocals 1 / k, k = 0..order + 2
+    align(4);
+    w += 4u * p->n_eq + pl.svout.size() + pl.sv_phase.size();
+    align(4);
+    bool elementary = false;
+    for (const auto &op : pl.ops) {
+        elementary = elementary || op.opcode < hb::detail::HY_FOP_FIRST;
+    }
+    out[0] = pl.n_slots;
+    out[1] = pl.n_gslots;
+    out[2] = static_cast<std::uint32_t>(pl.ops.size());
+    out[3] = pl.n_segments;
+    out[4] = elementary ? 1u : 0u;
+    out[5] = static_cast<std::uint32_t>((w + 3u) / 4u * 16u);
     return 0;
 }
 

@@ -22,7 +22,7 @@ SO = os.path.join(ROOT, "build", "libnb_emul.so")
 def _emul():
     src = os.path.join(ROOT, "tests", "cpp", "nb_emul.cpp")
     deps = [src, os.path.join(CSRC, "nb_core.hpp"), os.path.join(CSRC, "nb_plan.hpp"), os.path.join(CSRC, "nb_desc.hpp"),
-            os.path.join(CSRC, "nb_plan.cpp"),
+            os.path.join(CSRC, "nb_plan.cpp"), os.path.join(CSRC, "smem_plan.hpp"), os.path.join(CSRC, "smem_plan.cpp"),
             os.path.join(LIBDIR, "libheyoka_b200.so")]
     os.makedirs(os.path.dirname(SO), exist_ok=True)
     if not os.path.exists(SO) or os.path.getmtime(SO) < max(os.path.getmtime(d) for d in deps):

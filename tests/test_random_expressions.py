@@ -86,8 +86,9 @@ def build_case(seed):
 @pytest.mark.gpu
 @pytest.mark.parametrize("seed", range(16))
 def test_random_rhs_gpu_against_oracle(seed):
-    """The same random systems on the GPU (automatic kernel and the one-thread-per-lane kernel): one step with
-    write_tc and a short propagation against the oracle (no sympy on this path: the oracle is pinned on the CPU)."""
+    """The same random systems on the GPU (the automatic kernel, the HBM-tape kernel and the cooperative kernel with
+    its tape in global memory): one step with write_tc and a short propagation against the oracle (no sympy on this
+    path: the oracle is pinned on the CPU)."""
     sys_, _, _, ic = build_case(seed)
     P = hb.Program(sys_, tol=1e-12)
     for kernel in (dict(tape="auto"), dict(tape="hbm"), dict(tape="global")):
