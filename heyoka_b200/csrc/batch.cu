@@ -8,9 +8,11 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <initializer_list>
 #include <limits>
 #include <memory>
 #include <new>
+#include <optional>
 #include <stdexcept>
 #include <string>
 #include <thread>
@@ -181,6 +183,52 @@ std::size_t coop_warp_bytes(std::uint32_t n_slots, int L)
     return (static_cast<std::size_t>(n_slots) * l + 2u * l + (l + 1u) / 2u + 1u) / 2u * 2u * sizeof(double);
 }
 
+// Lets kernels take the largest dynamic shared memory the device allows. The attribute belongs to the function, for
+// the whole process: a value that depended on one batch would make the launches of another batch fail.
+template <typename F>
+void allow_max_smem(std::initializer_list<F> fns, std::size_t smem_optin)
+{
+    for (const F fn : fns) {
+        cudaFuncAttributes a{};
+        HY_CUDA_CHECK(cudaFuncGetAttributes(&a, fn));
+        HY_CUDA_CHECK(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                           static_cast<int>(smem_optin - a.sharedSizeBytes)));
+    }
+}
+
+// The kernel a batch runs: what hy_batch_get_kernel() reports (in the order of hy_kernel_info), the entry points, and
+// the sizes of the scratch the selection owns.
+struct kernel_sel {
+    enum family_t { hbm, coop, nb, nn } family = hbm;
+    int tape_mode = 0; // as hy_kernel_info::tape_mode reports it
+    int L = 0, N = 0;  // lanes per warp (team), lanes per thread
+    std::uint32_t threads = 0, per_sm = 0, grid = 0;
+    std::size_t smem = 0; // dynamic shared memory per CTA
+    std::uint32_t tape_slots = 0;
+    // Doubles of global scratch: the tape (k_hbm's slabs, the global or overflow tape of k_coop, k_nb's off-chip rows),
+    // and the private per-warp coefficient store (dev::coef_view).
+    std::size_t gscratch = 0, cscratch = 0;
+    const coop_variant *cv = nullptr;
+    const hy::detail::nb_variant *nbv = nullptr;
+};
+
+// The cooperative plan and its tables as one blob of 32-bit words.
+struct coop_tables {
+    hy::detail::smem_plan plan;
+    std::vector<std::uint32_t> blob;
+    std::size_t bytes = 0; // of the blob, rounded up to 16
+};
+
+// A decided selection and the host data its commit uploads (the commit fills in the device pointers of nbd and nnd).
+struct candidate {
+    kernel_sel k;
+    std::optional<coop_tables> tables; // a plan that replaces the batch's (with / without the overflow tape)
+    dev::nb_dev_plan nbd{};
+    std::vector<hy::detail::nb_role> nb_roles;
+    dev::nn_dev_plan nnd{};
+    std::vector<double> nn_wimg;
+};
+
 } // namespace
 
 // ------------------------------------------------------------------------------------------------
@@ -202,38 +250,27 @@ struct hy_batch {
     hy::detail::smem_plan plan;
     std::uint32_t *d_blob = nullptr;
     std::size_t blob_bytes = 0; // rounded up to 16 bytes
-    double *d_gscratch = nullptr; // overflow tape of the cooperative kernels (spilled private rows)
-    double *d_cscratch = nullptr; // private per-warp coefficient store of the cooperative kernels (see dev::coef_view)
     std::shared_ptr<const hy_program> prog_host; // kept for re-planning
     bool opt_fuse = true, opt_fuse_sv = true;
     int opt_spill = -1; // -1 automatic, 0 never, 1 always
-    void replan(bool spill);
+    coop_tables make_tables(bool spill) const;
+    void set_tables(coop_tables t);
     void ensure_tc();
-    void setup_coop_global(int L, int N, std::uint32_t threads, int cta = -1);
-    bool c_cta = false; // ... and the whole CTA working on one chunk of lanes (kernel mode 5)
-    bool c_global = false; // cooperative kernel with the tape in global memory (kernel mode 4)
-    // The dedicated N-body kernel (nb_kernel.cuh): plan, device copies of its tables, selected instantiation.
+    // The dedicated N-body kernel (nb_kernel.cuh): plan, device copies of its tables, device plan of the selected shape.
     hy::detail::nb_plan nbp;
     hy::detail::nb_pair_desc *d_nb_pairs = nullptr;
     hy::detail::nb_role *d_nb_roles = nullptr;
     std::uint32_t opt_nb_threads = 0; // HEYOKA_B200_NB_THREADS: preferred CTA size of the N-body kernel
     double *d_nb_consts = nullptr, *d_nb_fac = nullptr;
     dev::nb_dev_plan nbd{};
-    const hy::detail::nb_variant *nbv = nullptr;
-    coop_variant nb_cv{}; // (L, N, maxt, mode 6) of the selected N-body instantiation, for the code that reads cv->L
-    bool nb_on = false;
     int opt_nb = -1; // -1 automatic, 0 never (HEYOKA_B200_NB=0), 1 preferred
-    bool setup_nb(int LT, std::uint32_t threads, int want_cta, int want_lane = 0);
-    int opt_nb_lane = -1; // one thread per lane for single-pair systems: -1 automatic, 0 never (HEYOKA_B200_NB_LANE=0)
-    bool nb_lane = false;
+    int opt_nb1 = -1; // one thread per lane for single-pair systems: -1 automatic, 0 never (HEYOKA_B200_NB_LANE=0)
     // The dense-network kernel (nn_kernel.cuh): plan, padded weight image, device plan.
     hy::detail::nn_plan nnp;
     double *d_nn_wimg = nullptr;
     std::uint32_t *d_nn_out = nullptr;
     dev::nn_dev_plan nnd{};
-    bool nn_on = false;
     int opt_nn = -1; // 0: never (HEYOKA_B200_NN=0)
-    bool setup_nn();
 
     // Event detection (section E of the C ABI; ev_kernels.cuh). n_ev > 0: the program carries event equations, every
     // step is an event step (jet without propagation + detection + propagation cut at the first terminal event).
@@ -254,8 +291,8 @@ struct hy_batch {
     unsigned char *d_skip = nullptr; // per-lane mask of the masked zero-length step (propagate_finish())
 
     // Scratch.
-    double *d_scratch = nullptr; // per-warp tape slabs ("hbm" strategy only, allocated on demand)
-    std::size_t slab_doubles = 0;
+    double *d_gscratch = nullptr, *d_cscratch = nullptr; // the selection's (kernel_sel::gscratch, cscratch)
+    std::size_t slab_doubles = 0; // one warp's tape slab of k_hbm
     double *d_tmp = nullptr;      // 3 * n doubles: staged per-lane inputs (t_final hi/lo, max_delta_t)
     double *d_snapshot = nullptr; // state + time snapshot for the global-exit replay
     unsigned int *d_counter = nullptr;
@@ -264,11 +301,8 @@ struct hy_batch {
     // Kernel selection / launch geometry.
     std::uint32_t n_sms = 0;
     std::size_t smem_per_block_max = 0, smem_per_sm = 0;
-    int mode = 0;           // 1 = hbm, 2 = coop (resolved)
-    const coop_variant *cv = nullptr;
-    std::uint32_t c_threads = 0, c_grid = 0, c_ctas_per_sm = 0;
-    std::size_t c_smem = 0;
-    std::uint32_t h_threads = 256, h_blocks_per_sm = 0, h_grid = 0;
+    kernel_sel sel;
+    std::uint32_t h_threads = 256; // CTA size of k_hbm when a request gives none: the last one given
     std::uint64_t n_launches = 0;
 
     // Multi-device batch (hy_batch_create_multi()): the parent owns no device memory, only one single-device hy_batch
@@ -283,9 +317,15 @@ struct hy_batch {
     T *dalloc(std::size_t count);
     template <typename T>
     T *dupload(const std::vector<T> &v);
-    void configure(int want_mode, int L, int N, std::uint32_t threads, std::uint32_t blocks_per_sm);
-    void setup_hbm(std::uint32_t threads, std::uint32_t blocks_per_sm);
-    bool setup_coop(int L, int N, std::uint32_t threads, std::uint32_t ctas_per_sm);
+    // Kernel selection: decide() chooses without side effects on the batch, commit() installs the choice.
+    candidate decide(int want_mode, int L, int N, std::uint32_t threads, std::uint32_t blocks_per_sm) const;
+    void setup_hbm(std::uint32_t threads, std::uint32_t blocks_per_sm, candidate &c) const;
+    bool setup_coop(int L, int N, std::uint32_t threads, std::uint32_t ctas_per_sm, candidate &c) const;
+    void setup_coop_global(int L, int N, std::uint32_t threads, int cta, candidate &c) const;
+    bool setup_nb(int LT, std::uint32_t threads, int want_cta, int want_lane, candidate &c) const;
+    bool setup_nn(candidate &c) const;
+    std::size_t free_bytes_after_release() const;
+    void commit(candidate c);
     void launch(bool prop, const dev::run_args &R);
 };
 
@@ -319,7 +359,7 @@ void hy_batch::free_all() noexcept
           static_cast<void *>(d_tc), static_cast<void *>(d_d_out), static_cast<void *>(d_step_outcome),
           static_cast<void *>(d_prop_outcome), static_cast<void *>(d_prop_min_h), static_cast<void *>(d_prop_max_h),
           static_cast<void *>(d_prop_n_steps), static_cast<void *>(d_prop_iters), static_cast<void *>(d_skip),
-          static_cast<void *>(d_scratch), static_cast<void *>(d_tmp),
+          static_cast<void *>(d_tmp),
           static_cast<void *>(d_snapshot), static_cast<void *>(d_counter), static_cast<void *>(d_flags),
           static_cast<void *>(d_nb_pairs), static_cast<void *>(d_nb_roles), static_cast<void *>(d_nb_consts),
           static_cast<void *>(d_nb_fac), static_cast<void *>(d_nn_wimg), static_cast<void *>(d_nn_out)}) {
@@ -368,61 +408,66 @@ dev::batch hy_batch::view() const
     return b;
 }
 
-void hy_batch::setup_hbm(std::uint32_t threads, std::uint32_t blocks_per_sm)
+// Device memory that is free once the current selection's scratch is released.
+std::size_t hy_batch::free_bytes_after_release() const
 {
-    if (threads != 0u) {
-        if (threads % 32u != 0u || threads > 256u) {
-            throw std::invalid_argument("block_threads must be a multiple of 32 not larger than 256");
-        }
-        h_threads = threads;
+    std::size_t free_b = 0, total_b = 0;
+    HY_CUDA_CHECK(cudaMemGetInfo(&free_b, &total_b));
+    return free_b + (sel.gscratch + sel.cscratch) * sizeof(double);
+}
+
+void hy_batch::setup_hbm(std::uint32_t threads, std::uint32_t blocks_per_sm, candidate &c) const
+{
+    if (threads == 0u) {
+        threads = h_threads;
+    } else if (threads % 32u != 0u || threads > 256u) {
+        throw std::invalid_argument("block_threads must be a multiple of 32 not larger than 256");
     }
     if (blocks_per_sm == 0u) {
         int occ = 0;
         HY_CUDA_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, dev::k_hbm<true>,
-                                                                    static_cast<int>(h_threads), 0));
+                                                                    static_cast<int>(threads), 0));
         blocks_per_sm = static_cast<std::uint32_t>(std::max(occ, 1));
     }
-    h_blocks_per_sm = blocks_per_sm;
 
     // One slab per resident warp; never more warps than chunks of 32 lanes.
-    const std::uint32_t warps_per_block = h_threads / 32u;
+    const std::uint32_t warps_per_block = threads / 32u;
     const std::uint32_t n_chunks = (n + 31u) / 32u;
     const std::uint32_t needed_blocks = (n_chunks + warps_per_block - 1u) / warps_per_block;
-    h_grid = std::max(1u, std::min(n_sms * h_blocks_per_sm, needed_blocks));
-
-    if (d_scratch != nullptr) {
-        HY_CUDA_CHECK(cudaFree(d_scratch));
-        d_scratch = nullptr;
-    }
-    slab_doubles = static_cast<std::size_t>(n_uvars) * (order + 1u) * 32u;
     // The slabs of the resident warps must fit in (half of the free) device memory: large systems (model::ffnn
     // 3 x 64: 43 MB per warp) run with fewer resident blocks rather than failing to allocate.
-    {
-        std::size_t free_b = 0, total_b = 0;
-        HY_CUDA_CHECK(cudaMemGetInfo(&free_b, &total_b));
-        const std::size_t per_block = static_cast<std::size_t>(warps_per_block) * slab_doubles * sizeof(double);
-        const std::size_t max_blocks = std::max<std::size_t>(free_b / 2u / std::max<std::size_t>(per_block, 1u), 1u);
-        h_grid = static_cast<std::uint32_t>(std::min<std::size_t>(h_grid, max_blocks));
-    }
-    d_scratch = dalloc<double>(static_cast<std::size_t>(h_grid) * warps_per_block * slab_doubles);
-    mode = 1;
+    const std::size_t per_block = static_cast<std::size_t>(warps_per_block) * slab_doubles * sizeof(double);
+    const std::size_t max_blocks
+        = std::max<std::size_t>(free_bytes_after_release() / 2u / std::max<std::size_t>(per_block, 1u), 1u);
+    const auto grid = static_cast<std::uint32_t>(
+        std::min<std::size_t>(std::max(1u, std::min(n_sms * blocks_per_sm, needed_blocks)), max_blocks));
+    c.k = {kernel_sel::hbm, 1, 32, 1, threads, blocks_per_sm, grid, 0u, n_uvars * (order + 1u),
+           static_cast<std::size_t>(grid) * warps_per_block * slab_doubles};
 }
 
-void hy_batch::replan(bool spill)
+coop_tables hy_batch::make_tables(bool spill) const
 {
-    plan = hy::detail::make_smem_plan(*prog_host, opt_fuse, opt_fuse_sv, spill);
-    const auto blob = make_plan_blob(plan, *prog_host);
+    coop_tables t;
+    t.plan = hy::detail::make_smem_plan(*prog_host, opt_fuse, opt_fuse_sv, spill);
+    t.blob = make_plan_blob(t.plan, *prog_host);
+    t.bytes = (t.blob.size() + 3u) / 4u * 16u;
+    return t;
+}
+
+void hy_batch::set_tables(coop_tables t)
+{
     if (d_blob != nullptr) {
         HY_CUDA_CHECK(cudaFree(d_blob));
         d_blob = nullptr;
     }
-    d_blob = dupload(blob);
-    blob_bytes = (blob.size() + 3u) / 4u * 16u;
+    d_blob = dupload(t.blob);
+    blob_bytes = t.bytes;
+    plan = std::move(t.plan);
 }
 
 // Returns false if the requested / any configuration does not fit in shared memory.
 // L = lanes per warp, N = lanes per thread, threads = 32 x warps per block.
-bool hy_batch::setup_coop(int L, int N, std::uint32_t threads, std::uint32_t ctas_per_sm)
+bool hy_batch::setup_coop(int L, int N, std::uint32_t threads, std::uint32_t ctas_per_sm, candidate &c) const
 {
     const std::size_t reserve = 1024u; // per-block reservation of the driver
     if (N == 0) {
@@ -433,23 +478,21 @@ bool hy_batch::setup_coop(int L, int N, std::uint32_t threads, std::uint32_t cta
     // memory to global memory / L2, which lets 12 instead of 8 warps of the 6-body system reside on an SM.
     // Measured slower (1.89e7 vs 2.47e7 lane-steps/s: the L2 latency lands on the serial pow recurrence), hence
     // off by default; kept because it is what a system slightly too large for shared memory needs.
-    {
-        const bool have_spill = plan.n_gslots != 0u;
-        const bool want_spill = opt_spill > 0;
-        if (want_spill != have_spill) {
-            replan(want_spill);
-        }
+    if ((opt_spill > 0) != (plan.n_gslots != 0u)) {
+        c.tables = make_tables(opt_spill > 0);
     }
+    const auto &pl = c.tables ? c.tables->plan : plan;
+    const std::size_t blob_sz = c.tables ? c.tables->bytes : blob_bytes;
     if (L == 0) {
         // Lanes per warp: enough of them that an average dependency segment gives work to most of the
         // 32 threads (one work item = one u variable x N lanes), as long as at least 4 warps fit on an SM.
-        const double avg_width = static_cast<double>(plan.ops.size()) / std::max(1u, plan.n_segments);
+        const double avg_width = static_cast<double>(pl.ops.size()) / std::max(1u, pl.n_segments);
         for (const int cand : {1, 2, 4, 8, 16, 32}) {
             if (cand < N) {
                 continue;
             }
-            const auto bytes = coop_warp_bytes(plan.n_slots, cand);
-            if (blob_bytes + bytes + reserve > smem_per_block_max || (smem_per_sm - blob_bytes) / bytes < 4u) {
+            const auto bytes = coop_warp_bytes(pl.n_slots, cand);
+            if (blob_sz + bytes + reserve > smem_per_block_max || (smem_per_sm - blob_sz) / bytes < 4u) {
                 break;
             }
             L = cand;
@@ -459,7 +502,7 @@ bool hy_batch::setup_coop(int L, int N, std::uint32_t threads, std::uint32_t cta
         }
         if (L == 0) {
             // Not even 4 warps of the smallest shape fit: take whatever fits at all.
-            if (blob_bytes + coop_warp_bytes(plan.n_slots, N) + reserve > smem_per_block_max) {
+            if (blob_sz + coop_warp_bytes(pl.n_slots, N) + reserve > smem_per_block_max) {
                 return false;
             }
             L = N;
@@ -468,18 +511,18 @@ bool hy_batch::setup_coop(int L, int N, std::uint32_t threads, std::uint32_t cta
     // Warps per CTA that fit next to one copy of the tables (at most 16).
     const auto fit_warps = [&](std::uint32_t n_slots, int lanes) -> std::size_t {
         const auto wb = coop_warp_bytes(n_slots, lanes);
-        if (blob_bytes + wb + reserve > smem_per_block_max) {
+        if (blob_sz + wb + reserve > smem_per_block_max) {
             return 0u;
         }
-        return std::min<std::size_t>((smem_per_block_max - reserve - blob_bytes) / wb, 16u);
+        return std::min<std::size_t>((smem_per_block_max - reserve - blob_sz) / wb, 16u);
     };
-    const auto warp_bytes = coop_warp_bytes(plan.n_slots, L);
-    if (blob_bytes > 24u * 1024u || blob_bytes + warp_bytes + reserve > smem_per_block_max) {
+    const auto warp_bytes = coop_warp_bytes(pl.n_slots, L);
+    if (blob_sz > 24u * 1024u || blob_sz + warp_bytes + reserve > smem_per_block_max) {
         return false;
     }
     if (threads == 0u) {
         // One CTA per SM holding as many warps as fit in shared memory.
-        const std::size_t W = fit_warps(plan.n_slots, L);
+        const std::size_t W = fit_warps(pl.n_slots, L);
         threads = static_cast<std::uint32_t>(32u * std::max<std::size_t>(W, 1u));
     }
     if (threads % 32u != 0u || threads == 0u || threads > 512u) {
@@ -487,7 +530,7 @@ bool hy_batch::setup_coop(int L, int N, std::uint32_t threads, std::uint32_t cta
     }
     // Registers: 65536 / 512 threads = 128 per thread, 170 with at most 384 threads, 255 with at most 256.
     int kmode = 0;
-    for (const auto &op : plan.ops) {
+    for (const auto &op : pl.ops) {
         kmode = op.opcode < hy::detail::HY_FOP_FIRST ? 1 : kmode;
     }
     // (Not every shape is compiled for every CTA size: fall back to the next larger bound.)
@@ -502,40 +545,22 @@ bool hy_batch::setup_coop(int L, int N, std::uint32_t threads, std::uint32_t cta
         throw std::invalid_argument("Unsupported cooperative kernel configuration: " + std::to_string(L)
                                     + " lanes per warp, " + std::to_string(N) + " lanes per thread");
     }
-    const std::size_t bytes = blob_bytes + static_cast<std::size_t>(threads / 32u) * warp_bytes;
+    const std::size_t bytes = blob_sz + static_cast<std::size_t>(threads / 32u) * warp_bytes;
     if (bytes + reserve > smem_per_block_max) {
         return false;
     }
-    for (auto fn : {v->step, v->prop}) {
-        HY_CUDA_CHECK(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(bytes)));
-    }
+    allow_max_smem({v->step, v->prop}, smem_per_block_max);
     if (ctas_per_sm == 0u) {
         int occ = 0;
         HY_CUDA_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, v->prop, static_cast<int>(threads), bytes));
         ctas_per_sm = static_cast<std::uint32_t>(std::max(occ, 1));
     }
-    if (d_gscratch != nullptr) {
-        HY_CUDA_CHECK(cudaFree(d_gscratch));
-        d_gscratch = nullptr;
-    }
-    if (d_cscratch != nullptr) {
-        HY_CUDA_CHECK(cudaFree(d_cscratch));
-        d_cscratch = nullptr;
-    }
-    cv = v;
-    c_threads = threads;
-    c_smem = bytes;
-    c_ctas_per_sm = ctas_per_sm;
     const std::uint32_t lanes_per_block = static_cast<std::uint32_t>(L) * (threads / 32u);
     const std::uint32_t n_blocks_needed = (n + lanes_per_block - 1u) / lanes_per_block;
-    c_grid = std::max(1u, std::min(n_sms * ctas_per_sm, n_blocks_needed));
-    if (plan.n_gslots != 0u) {
-        d_gscratch = dalloc<double>(static_cast<std::size_t>(c_grid) * (threads / 32u) * plan.n_gslots
-                                    * static_cast<std::size_t>(L));
-    }
-    d_cscratch = dalloc<double>(static_cast<std::size_t>(c_grid) * (threads / 32u) * (order + 1u) * n_eq
-                                * static_cast<std::size_t>(L));
-    mode = 2;
+    const std::uint32_t grid = std::max(1u, std::min(n_sms * ctas_per_sm, n_blocks_needed));
+    const std::size_t warp_lanes = static_cast<std::size_t>(grid) * (threads / 32u) * static_cast<std::size_t>(L);
+    c.k = {kernel_sel::coop, 2, L, N, threads, ctas_per_sm, grid, bytes, pl.n_slots, warp_lanes * pl.n_gslots,
+           warp_lanes * (order + 1u) * n_eq, v};
     return true;
 }
 
@@ -543,11 +568,13 @@ bool hy_batch::setup_coop(int L, int N, std::uint32_t threads, std::uint32_t cta
 // bodies: 56k doubles per lane): same program, same planner, but every warp's tape is a slab of global memory and
 // the tables are read in place. Unlike the one-thread-per-lane HBM-tape kernel it fills the GPU with a few
 // thousand lanes (a warp works on L lanes, its threads on different u variables).
-void hy_batch::setup_coop_global(int L, int N, std::uint32_t threads, int cta)
+void hy_batch::setup_coop_global(int L, int N, std::uint32_t threads, int cta, candidate &c) const
 {
+    c.tables.reset();
     if (plan.n_gslots != 0u) {
-        replan(false);
+        c.tables = make_tables(false);
     }
+    const auto &pl = c.tables ? c.tables->plan : plan;
     if (N == 0) {
         N = (L == 0 || L >= 2) ? 2 : 1;
     }
@@ -563,7 +590,7 @@ void hy_batch::setup_coop_global(int L, int N, std::uint32_t threads, int cta)
         // threads and there are too few lanes to keep every warp of the GPU busy for long: the lane-step latency
         // drops by the number of warps (a slow lane no longer holds the launch), and the tapes in flight
         // (n_sms x L lanes) nearly fit in L2. Otherwise one warp per chunk (mode 4).
-        const double avg_width = static_cast<double>(plan.ops.size()) / std::max(1u, plan.n_segments);
+        const double avg_width = static_cast<double>(pl.ops.size()) / std::max(1u, pl.n_segments);
         const std::uint64_t warp_chunks = (n + static_cast<std::uint32_t>(N) - 1u) / static_cast<std::uint32_t>(N);
         cta = (avg_width >= 128. && warp_chunks < 8ull * n_sms * warps) ? 1 : 0;
     }
@@ -582,32 +609,17 @@ void hy_batch::setup_coop_global(int L, int N, std::uint32_t threads, int cta)
                                     + std::to_string(L) + " lanes per warp, " + std::to_string(N)
                                     + " lanes per thread");
     }
-    for (double **ptr : {&d_gscratch, &d_cscratch}) {
-        if (*ptr != nullptr) {
-            HY_CUDA_CHECK(cudaFree(*ptr));
-            *ptr = nullptr;
-        }
-    }
     // Teams (warps, or whole CTAs) per block, each with its own slab and private coefficient store.
     const std::uint32_t teams = cta != 0 ? 1u : warps;
-    const std::size_t team_bytes = coop_warp_bytes(plan.n_slots, L);
+    const std::size_t team_bytes = coop_warp_bytes(pl.n_slots, L);
     const std::uint32_t lanes_per_block = static_cast<std::uint32_t>(L) * teams;
     const std::uint32_t n_blocks_needed = (n + lanes_per_block - 1u) / lanes_per_block;
-    std::size_t free_b = 0, total_b = 0;
-    HY_CUDA_CHECK(cudaMemGetInfo(&free_b, &total_b));
-    const std::size_t max_blocks = std::max<std::size_t>(free_b / 2u / (team_bytes * teams), 1u);
-    cv = v;
-    c_threads = threads;
-    c_smem = 0;
-    c_ctas_per_sm = 1;
-    c_grid = static_cast<std::uint32_t>(
+    const std::size_t max_blocks = std::max<std::size_t>(free_bytes_after_release() / 2u / (team_bytes * teams), 1u);
+    const auto grid = static_cast<std::uint32_t>(
         std::max<std::size_t>(1u, std::min<std::size_t>({n_sms, n_blocks_needed, max_blocks})));
-    d_gscratch = dalloc<double>(static_cast<std::size_t>(c_grid) * teams * (team_bytes / sizeof(double)));
-    d_cscratch = dalloc<double>(static_cast<std::size_t>(c_grid) * teams * (order + 1u) * n_eq
-                                * static_cast<std::size_t>(L));
-    mode = 2;
-    c_global = true;
-    c_cta = cta != 0;
+    const std::size_t team_count = static_cast<std::size_t>(grid) * teams;
+    c.k = {kernel_sel::coop, cta != 0 ? 5 : 4, L, N, threads, 1u, grid, 0u, pl.n_slots,
+           team_count * (team_bytes / sizeof(double)), team_count * (order + 1u) * n_eq * L, v};
 }
 
 // The table of the one-thread-per-lane N-body kernel (nb1_kernel.cuh) for a plan with ONE pair interaction whose six
@@ -673,7 +685,7 @@ static bool make_nb1_tab(const hy::detail::nb_plan &pl, std::uint32_t n_eq, std:
 // The dedicated N-body kernel. LT = lanes per team (0: as many as give every thread of a warp one pair interaction),
 // threads = CTA size (0: as many warps as fit; HEYOKA_B200_NB_THREADS caps it), want_cta: -1 automatic.
 // Returns false if the program does not qualify or nothing fits.
-bool hy_batch::setup_nb(int LT, std::uint32_t threads, int want_cta, int want_lane)
+bool hy_batch::setup_nb(int LT, std::uint32_t threads, int want_cta, int want_lane, candidate &c) const
 {
     if (!nbp.ok) {
         return false;
@@ -794,75 +806,40 @@ bool hy_batch::setup_nb(int LT, std::uint32_t threads, int want_cta, int want_la
     if (v == nullptr) {
         return false;
     }
-    // Device copies of the tables.
-    if (d_nb_pairs == nullptr) {
-        d_nb_pairs = dupload(nbp.pairs);
-        d_nb_consts = dupload(nbp.consts);
-        d_nb_fac = dupload(nbp.fac);
-    }
-    if (d_nb_roles != nullptr) {
-        HY_CUDA_CHECK(cudaFree(d_nb_roles));
-        d_nb_roles = nullptr;
-    }
-    d_nb_roles = dupload(roles.table);
-    nbd = dev::nb_dev_plan{};
-    nbd.pairs = d_nb_pairs;
-    nbd.roles = reinterpret_cast<const uint4 *>(d_nb_roles);
-    nbd.consts = d_nb_consts;
-    nbd.fac = d_nb_fac;
-    nbd.n_pairs = n_pairs;
-    nbd.n_pos = nbp.n_pos;
-    nbd.n_out = nbp.n_out;
-    nbd.n_consts = static_cast<std::uint32_t>(nbp.consts.size());
-    nbd.npp = npp;
-    nbd.fac_stride = nbp.fac_stride;
-    nbd.n_rounds = roles.n_rounds;
-    nbd.round_level_end = roles.round_level_end;
-    nbd.alpha = nbp.alpha;
-    nbd.pow_algo = nbp.pow_algo;
-    nbd.roles_in_smem = pick.roles_in_smem ? 1u : 0u;
-    nbd.shared_doubles = static_cast<std::uint32_t>(shared_doubles(pick.roles_in_smem));
-    nbd.n_slots_equiv = team_slots(pick.offchip);
-    nbd.l1 = l1;
-    nb_lane = lane;
-    const std::size_t team_bytes = coop_warp_bytes(nbd.n_slots_equiv, LT);
-    nbd.team_doubles = static_cast<std::uint32_t>(team_bytes / sizeof(double));
+    dev::nb_dev_plan &d = c.nbd;
+    d.n_pairs = n_pairs;
+    d.n_pos = nbp.n_pos;
+    d.n_out = nbp.n_out;
+    d.n_consts = static_cast<std::uint32_t>(nbp.consts.size());
+    d.npp = npp;
+    d.fac_stride = nbp.fac_stride;
+    d.n_rounds = roles.n_rounds;
+    d.round_level_end = roles.round_level_end;
+    d.alpha = nbp.alpha;
+    d.pow_algo = nbp.pow_algo;
+    d.roles_in_smem = pick.roles_in_smem ? 1u : 0u;
+    d.shared_doubles = static_cast<std::uint32_t>(shared_doubles(pick.roles_in_smem));
+    d.n_slots_equiv = team_slots(pick.offchip);
+    d.l1 = l1;
+    const std::size_t team_bytes = coop_warp_bytes(d.n_slots_equiv, LT);
+    d.team_doubles = static_cast<std::uint32_t>(team_bytes / sizeof(double));
+    c.nb_roles = std::move(roles.table);
     const std::uint32_t teams = cta ? 1u : threads / 32u;
-    const std::size_t bytes = static_cast<std::size_t>(nbd.shared_doubles) * sizeof(double) + teams * team_bytes;
-    for (auto fn : {v->step, v->prop}) {
-        HY_CUDA_CHECK(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(bytes)));
-    }
-    for (double **ptr : {&d_gscratch, &d_cscratch}) {
-        if (*ptr != nullptr) {
-            HY_CUDA_CHECK(cudaFree(*ptr));
-            *ptr = nullptr;
-        }
-    }
-    nbv = v;
-    nb_cv = coop_variant{LT, LT >= 2 ? 2 : 1, v->maxt, cta ? 7 : 6, nullptr, nullptr};
-    cv = &nb_cv;
-    c_threads = threads;
-    c_smem = bytes;
-    c_ctas_per_sm = 1;
+    const std::size_t bytes = static_cast<std::size_t>(d.shared_doubles) * sizeof(double) + teams * team_bytes;
+    allow_max_smem({v->step, v->prop}, smem_per_block_max);
     const std::uint32_t lanes_per_block = static_cast<std::uint32_t>(LT) * teams;
     const std::uint32_t n_blocks_needed = (n + lanes_per_block - 1u) / lanes_per_block;
-    c_grid = std::max(1u, std::min(n_sms, n_blocks_needed));
-    d_cscratch = dalloc<double>(static_cast<std::size_t>(c_grid) * teams * (order + 1u) * n_eq
-                                * static_cast<std::size_t>(LT));
-    if (pick.offchip) {
-        d_gscratch = dalloc<double>(static_cast<std::size_t>(c_grid) * npp * 3u * TT * 2u);
-        nbd.offchip = d_gscratch;
-    }
-    mode = 2;
-    nb_on = true;
-    c_cta = cta;
+    const std::uint32_t grid = std::max(1u, std::min(n_sms, n_blocks_needed));
+    c.k = {kernel_sel::nb, lane ? 9 : (cta ? 7 : 6), LT, LT >= 2 ? 2 : 1, threads, 1u, grid, bytes, d.n_slots_equiv,
+           pick.offchip ? static_cast<std::size_t>(grid) * npp * 3u * TT * 2u : 0u,
+           static_cast<std::size_t>(grid) * teams * (order + 1u) * n_eq * static_cast<std::size_t>(LT), nullptr, v};
     return true;
 }
 
 // The dense-network kernel: the padded shared-memory image of the weights is prepared here (row pitch = 4 mod 16
 // doubles: the 8 x 4 A fragments of the tensor-core products then read conflict-free), copied once per CTA by the TMA
 // unit. Returns false if the program is not a network or does not fit in shared memory.
-bool hy_batch::setup_nn()
+bool hy_batch::setup_nn(candidate &c) const
 {
     if (!nnp.ok || nnp.layers.size() > static_cast<std::size_t>(dev::NN_MAX_LAYERS)) {
         return false;
@@ -908,50 +885,24 @@ bool hy_batch::setup_nn()
     if (bytes + 2048u > smem_per_block_max) {
         return false;
     }
-    for (void **ptr : {reinterpret_cast<void **>(&d_nn_wimg), reinterpret_cast<void **>(&d_nn_out)}) {
-        if (*ptr != nullptr) {
-            HY_CUDA_CHECK(cudaFree(*ptr));
-            *ptr = nullptr;
-        }
-    }
-    d_nn_wimg = dupload(img);
-    d_nn_out = dupload(nnp.out_of_sv);
-    d.wimg = d_nn_wimg;
-    d.out_of_sv = d_nn_out;
-    nnd = d;
-    for (auto fn : {hy::detail::nn_kernel_step(), hy::detail::nn_kernel_prop()}) {
-        HY_CUDA_CHECK(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(bytes)));
-    }
-    for (double **ptr : {&d_gscratch, &d_cscratch}) {
-        if (*ptr != nullptr) {
-            HY_CUDA_CHECK(cudaFree(*ptr));
-            *ptr = nullptr;
-        }
-    }
-    nb_cv = coop_variant{dev::NN_LB, 1, dev::NN_THREADS, 8, nullptr, nullptr};
-    cv = &nb_cv;
-    c_threads = dev::NN_THREADS;
-    c_smem = bytes;
-    c_ctas_per_sm = 1;
-    const std::uint32_t n_blocks_needed = (n + dev::NN_LB - 1u) / dev::NN_LB;
-    c_grid = std::max(1u, std::min(n_sms, n_blocks_needed));
-    mode = 2;
-    nn_on = true;
+    allow_max_smem({hy::detail::nn_kernel_step(), hy::detail::nn_kernel_prop()}, smem_per_block_max);
+    c.nnd = d;
+    c.nn_wimg = std::move(img);
+    const std::uint32_t grid = std::max(1u, std::min(n_sms, (n + dev::NN_LB - 1u) / dev::NN_LB));
+    c.k = {kernel_sel::nn, 8, dev::NN_LB, 1, dev::NN_THREADS, 1u, grid, bytes, plan.n_slots};
     return true;
 }
 
-void hy_batch::configure(int want_mode, int L, int N, std::uint32_t threads, std::uint32_t blocks_per_sm)
+// The kernel a request selects (tape_mode as hy_batch_set_kernel() takes it, 0 automatic). A request that cannot run
+// throws, and leaves the batch as it is.
+candidate hy_batch::decide(int want_mode, int L, int N, std::uint32_t threads, std::uint32_t blocks_per_sm) const
 {
-    c_global = false;
-    c_cta = false;
-    nb_on = false;
-    nb_lane = false;
-    nn_on = false;
+    candidate c;
     // Mode 8: the dense-network kernel (right-hand sides that are feed-forward networks, nn_plan.hpp); the automatic
     // mode takes it whenever the program qualifies.
     if (want_mode == 8 || (want_mode == 0 && opt_nn != 0)) {
-        if (setup_nn()) {
-            return;
+        if (setup_nn(c)) {
+            return c;
         }
         if (want_mode == 8) {
             throw std::invalid_argument("The dense-network kernel cannot run this program: "
@@ -963,9 +914,9 @@ void hy_batch::configure(int want_mode, int L, int N, std::uint32_t threads, std
     if (want_mode == 6 || want_mode == 7 || want_mode == 9 || (want_mode == 0 && opt_nb != 0)) {
         // Mode 9: one thread per lane (systems with one pair interaction); the automatic mode takes it when it applies,
         // an explicit mode 6 never does (it selects k_nb with the given team shape).
-        const int want_lane = want_mode == 9 ? 1 : (want_mode == 0 ? (opt_nb_lane != 0 ? -1 : 0) : 0);
-        if (setup_nb(want_mode == 9 ? 32 : L, threads, want_mode == 0 ? -1 : (want_mode == 7 ? 1 : 0), want_lane)) {
-            return;
+        const int lane = want_mode == 9 ? 1 : (want_mode == 0 ? (opt_nb1 != 0 ? -1 : 0) : 0);
+        if (setup_nb(want_mode == 9 ? 32 : L, threads, want_mode == 0 ? -1 : (want_mode == 7 ? 1 : 0), lane, c)) {
+            return c;
         }
         if (want_mode != 0) {
             throw std::invalid_argument("The N-body kernel cannot run this program: "
@@ -973,25 +924,72 @@ void hy_batch::configure(int want_mode, int L, int N, std::uint32_t threads, std
         }
     }
     if (want_mode == 4 || want_mode == 5) {
-        setup_coop_global(L, N, threads, want_mode == 5 ? 1 : 0);
-        return;
+        setup_coop_global(L, N, threads, want_mode == 5 ? 1 : 0, c);
+        return c;
     }
     if (want_mode == 1) {
-        setup_hbm(threads, blocks_per_sm);
-        return;
+        setup_hbm(threads, blocks_per_sm, c);
+        return c;
     }
     if (want_mode == 3) {
         want_mode = 2;
     }
-    if (setup_coop(L, N, threads, blocks_per_sm)) {
-        return;
+    if (setup_coop(L, N, threads, blocks_per_sm, c)) {
+        return c;
     }
     if (want_mode == 2) {
-        throw std::invalid_argument("The derivative tape of this system (" + std::to_string(plan.n_slots)
+        throw std::invalid_argument("The derivative tape of this system ("
+                                    + std::to_string((c.tables ? c.tables->plan : plan).n_slots)
                                     + " doubles per lane) does not fit in shared memory");
     }
     // Automatic: the cooperative kernel with the tape in global memory.
-    setup_coop_global(0, 0, 0);
+    setup_coop_global(0, 0, 0, -1, c);
+    return c;
+}
+
+// Installs a decided selection: releases the scratch of the current one, uploads the tables of the new one and
+// allocates its scratch. Only CUDA errors can fail here.
+void hy_batch::commit(candidate c)
+{
+    const auto release = [](auto *&p) {
+        if (p != nullptr) {
+            HY_CUDA_CHECK(cudaFree(p));
+            p = nullptr;
+        }
+    };
+    release(d_gscratch);
+    release(d_cscratch);
+    release(d_nb_roles);
+    release(d_nn_wimg);
+    release(d_nn_out);
+    if (c.tables) {
+        set_tables(std::move(*c.tables));
+    }
+    d_gscratch = c.k.gscratch != 0u ? dalloc<double>(c.k.gscratch) : nullptr;
+    d_cscratch = c.k.cscratch != 0u ? dalloc<double>(c.k.cscratch) : nullptr;
+    if (c.k.family == kernel_sel::hbm) {
+        h_threads = c.k.threads;
+    } else if (c.k.family == kernel_sel::nb) {
+        if (d_nb_pairs == nullptr) {
+            d_nb_pairs = dupload(nbp.pairs);
+            d_nb_consts = dupload(nbp.consts);
+            d_nb_fac = dupload(nbp.fac);
+        }
+        d_nb_roles = dupload(c.nb_roles);
+        nbd = c.nbd;
+        nbd.pairs = d_nb_pairs;
+        nbd.roles = reinterpret_cast<const uint4 *>(d_nb_roles);
+        nbd.consts = d_nb_consts;
+        nbd.fac = d_nb_fac;
+        nbd.offchip = d_gscratch;
+    } else if (c.k.family == kernel_sel::nn) {
+        d_nn_wimg = dupload(c.nn_wimg);
+        d_nn_out = dupload(nnp.out_of_sv);
+        nnd = c.nnd;
+        nnd.wimg = d_nn_wimg;
+        nnd.out_of_sv = d_nn_out;
+    }
+    sel = c.k;
 }
 
 // The public Taylor-coefficient array, [n_eq][order + 1][batch] (src/taylor_00.cpp:574-580), is allocated the first
@@ -1081,8 +1079,8 @@ void hy_batch::ev_step(const double *d_mdt, int, int backward)
     if (!ev_set) {
         throw std::invalid_argument("hy_batch_set_events() must be called before stepping a batch with event equations");
     }
-    if (mode != 1 || d_scratch == nullptr) {
-        setup_hbm(0, 0);
+    if (sel.family != kernel_sel::hbm) {
+        commit(decide(1, 0, 0, 0, 0));
     }
     ensure_tc();
     const std::uint32_t B = n;
@@ -1092,7 +1090,7 @@ void hy_batch::ev_step(const double *d_mdt, int, int backward)
     R.counter = d_counter;
     R.flags = d_flags;
     HY_CUDA_CHECK(cudaMemsetAsync(d_counter, 0, sizeof(unsigned int), stream));
-    dev::k_ev_jet<<<h_grid, h_threads, 0, stream>>>(prog, view(), R, eva, d_scratch, slab_doubles);
+    dev::k_ev_jet<<<sel.grid, sel.threads, 0, stream>>>(prog, view(), R, eva, d_gscratch, slab_doubles);
     HY_CUDA_CHECK(cudaGetLastError());
     n_launches += 1;
     unsigned counters[4] = {0u, 0u, 0u, 0u};
@@ -1161,38 +1159,40 @@ void hy_batch::ev_step(const double *d_mdt, int, int backward)
 
 void hy_batch::launch(bool prop, const dev::run_args &R)
 {
-    if (R.write_tc != 0 || (mode == 2 && d_cscratch == nullptr && !nn_on)) {
+    if (R.write_tc != 0) {
         ensure_tc();
     }
     HY_CUDA_CHECK(cudaMemsetAsync(d_counter, 0, sizeof(unsigned int), stream));
-    if (nn_on) {
-        (prop ? hy::detail::nn_kernel_prop() : hy::detail::nn_kernel_step())<<<c_grid, c_threads, c_smem, stream>>>(
+    const kernel_sel &k = sel;
+    switch (k.family) {
+    case kernel_sel::hbm:
+        (prop ? dev::k_hbm<true> : dev::k_hbm<false>)<<<k.grid, k.threads, 0, stream>>>(prog, view(), R, d_gscratch,
+                                                                                        slab_doubles);
+        break;
+    case kernel_sel::nn:
+        (prop ? hy::detail::nn_kernel_prop() : hy::detail::nn_kernel_step())<<<k.grid, k.threads, k.smem, stream>>>(
             prog, nnd, view(), R);
-    } else if (mode == 2) {
+        break;
+    case kernel_sel::coop:
+    case kernel_sel::nb: {
+        // The coefficients of a step go to the private per-warp store, or to tc on request. k_nb1 always works on its
+        // private store ([order][slot][32 lanes], velocities only) and publishes the coefficients to tc on request.
         dev::run_args R2 = R;
-        const bool pub = R.write_tc != 0 || d_cscratch == nullptr;
-        const auto lanes = static_cast<unsigned long long>(cv->L);
+        const bool pub = R.write_tc != 0, priv = !pub || k.tape_mode == 9;
+        const auto lanes = static_cast<unsigned long long>(k.L);
         R2.coef_pub = pub ? 1 : 0;
-        R2.coef_base = pub ? d_tc : d_cscratch;
-        R2.coef_warp_stride = pub ? 0ull : static_cast<unsigned long long>(order + 1u) * n_eq * lanes;
+        R2.coef_base = priv ? d_cscratch : d_tc;
+        R2.coef_warp_stride = priv ? static_cast<unsigned long long>(order + 1u) * n_eq * lanes : 0ull;
         R2.coef_stride_sv = pub ? static_cast<unsigned long long>(order + 1u) * n : lanes;
         R2.coef_stride_o = pub ? static_cast<unsigned long long>(n) : static_cast<unsigned long long>(n_eq) * lanes;
-        if (nb_on && nb_lane) {
-            // k_nb1 always works on its private store ([order][slot][32 lanes], velocities only) and publishes the
-            // coefficients to tc on request.
-            R2.coef_base = d_cscratch;
-            R2.coef_warp_stride = static_cast<unsigned long long>(order + 1u) * n_eq * lanes;
-            R2.coef_pub = R.write_tc != 0 ? 1 : 0;
-        }
-        if (nb_on) {
-            (prop ? nbv->prop : nbv->step)<<<c_grid, c_threads, c_smem, stream>>>(prog, nbd, view(), R2);
+        if (k.family == kernel_sel::nb) {
+            (prop ? k.nbv->prop : k.nbv->step)<<<k.grid, k.threads, k.smem, stream>>>(prog, nbd, view(), R2);
         } else {
-            (prop ? cv->prop : cv->step)<<<c_grid, c_threads, c_smem, stream>>>(prog, d_blob, view(), R2, d_gscratch);
+            (prop ? k.cv->prop : k.cv->step)<<<k.grid, k.threads, k.smem, stream>>>(prog, d_blob, view(), R2,
+                                                                                    d_gscratch);
         }
-    } else if (prop) {
-        dev::k_hbm<true><<<h_grid, h_threads, 0, stream>>>(prog, view(), R, d_scratch, slab_doubles);
-    } else {
-        dev::k_hbm<false><<<h_grid, h_threads, 0, stream>>>(prog, view(), R, d_scratch, slab_doubles);
+        break;
+    }
     }
     HY_CUDA_CHECK(cudaGetLastError());
     ++n_launches;
@@ -1514,13 +1514,14 @@ int hy_batch_create(const hy_program *p, uint32_t batch, int device, hy_batch **
             b->opt_nb = std::string{env} != "0" ? 1 : 0;
         }
         if (const char *env = std::getenv("HEYOKA_B200_NB_LANE")) {
-            b->opt_nb_lane = std::string{env} != "0" ? 1 : 0;
+            b->opt_nb1 = std::string{env} != "0" ? 1 : 0;
         }
         if (const char *env = std::getenv("HEYOKA_B200_NB_THREADS")) {
             b->opt_nb_threads = static_cast<std::uint32_t>(std::atoi(env));
         }
         b->prog_host = std::make_shared<const hy_program>(*p);
-        b->replan(false);
+        b->set_tables(b->make_tables(false));
+        b->slab_doubles = static_cast<std::size_t>(p->n_uvars) * (p->order + 1u) * 32u;
         b->nbp = hy::detail::make_nb_plan(*p);
         if (const char *env = std::getenv("HEYOKA_B200_NN")) {
             b->opt_nn = std::string{env} != "0" ? 1 : 0;
@@ -1568,7 +1569,7 @@ int hy_batch_create(const hy_program *p, uint32_t batch, int device, hy_batch **
             }
             want = 1;
         }
-        b->configure(want, 0, 0, 0, 0);
+        b->commit(b->decide(want, 0, 0, 0, 0));
 
         *out = b;
         return HY_OK;
@@ -1736,15 +1737,10 @@ int hy_batch_set_launch_config(hy_batch *b, uint32_t block_threads, uint32_t blo
         }
         device_guard guard(b->device);
         HY_CUDA_CHECK(cudaStreamSynchronize(b->stream));
-        const int L = b->cv != nullptr && b->mode == 2 ? b->cv->L : 0;
-        const int N = b->cv != nullptr && b->mode == 2 ? b->cv->N : 0;
-        if (b->nn_on) {
-            b->configure(8, 0, 0, 0, 0);
-        } else if (b->nb_on) {
-            b->configure(b->nb_lane ? 9 : (b->c_cta ? 7 : 6), L, 0, block_threads, blocks_per_sm);
-        } else {
-            b->configure(b->mode, L, N, block_threads, blocks_per_sm);
-        }
+        // The same tape mode and lanes (the N-body kernels derive their lanes per thread from the team; the network
+        // kernel has a fixed shape and ignores every argument).
+        const kernel_sel &k = b->sel;
+        b->commit(b->decide(k.tape_mode, k.L, k.family == kernel_sel::nb ? 0 : k.N, block_threads, blocks_per_sm));
         return HY_OK;
     } catch (...) {
         return translate_exception();
@@ -1772,8 +1768,8 @@ int hy_batch_set_kernel(hy_batch *b, int tape_mode, uint32_t lanes_per_warp, uin
         }
         device_guard guard(b->device);
         HY_CUDA_CHECK(cudaStreamSynchronize(b->stream));
-        b->configure(tape_mode, static_cast<int>(lanes_per_warp), static_cast<int>(lanes_per_thread), block_threads,
-                     blocks_per_sm);
+        b->commit(b->decide(tape_mode, static_cast<int>(lanes_per_warp), static_cast<int>(lanes_per_thread),
+                            block_threads, blocks_per_sm));
         return HY_OK;
     } catch (...) {
         return translate_exception();
@@ -1789,14 +1785,15 @@ int hy_batch_get_kernel(const hy_batch *b, hy_kernel_info *out)
     if (!b->shards.empty()) {
         return hy_batch_get_kernel(b->shards[0], out); // (every shard runs the same kernel shape)
     }
-    out->tape_mode = b->nn_on ? 8 : b->nb_on ? (b->nb_lane ? 9 : (b->c_cta ? 7 : 6)) : (b->mode == 2 && b->c_global ? (b->c_cta ? 5 : 4) : b->mode);
-    out->lanes_per_warp = b->mode == 2 ? static_cast<uint32_t>(b->cv->L) : 32u;
-    out->lanes_per_thread = b->mode == 2 ? static_cast<uint32_t>(b->cv->N) : 1u;
-    out->block_threads = b->mode == 2 ? b->c_threads : b->h_threads;
-    out->blocks_per_sm = b->mode == 2 ? b->c_ctas_per_sm : b->h_blocks_per_sm;
-    out->grid = b->mode == 2 ? b->c_grid : b->h_grid;
-    out->smem_bytes = b->mode == 2 ? static_cast<uint64_t>(b->c_smem) : 0u;
-    out->tape_slots_per_lane = b->nb_on ? b->nbd.n_slots_equiv : (b->mode == 2 ? b->plan.n_slots : b->n_uvars * (b->order + 1u));
+    const kernel_sel &k = b->sel;
+    out->tape_mode = k.tape_mode;
+    out->lanes_per_warp = static_cast<uint32_t>(k.L);
+    out->lanes_per_thread = static_cast<uint32_t>(k.N);
+    out->block_threads = k.threads;
+    out->blocks_per_sm = k.per_sm;
+    out->grid = k.grid;
+    out->smem_bytes = k.smem;
+    out->tape_slots_per_lane = k.tape_slots;
     out->n_segments = b->plan.n_segments;
     out->n_fused = b->plan.n_fused;
     out->n_sms = b->n_sms;

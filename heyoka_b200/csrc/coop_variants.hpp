@@ -21,7 +21,8 @@ using coop_fn = void (*)(dev::program, const std::uint32_t *, dev::batch, dev::r
 
 struct coop_variant {
     int L, N, maxt; // lanes per warp, lanes per thread, maximum threads per CTA
-    int mode;       // 1: handles elementary ops, 0: superinstruction-only programs, 4: tape in global memory, 5: idem, CTA-wide teams
+    int mode;       // HY_COOP_MODE (not hy_kernel_info::tape_mode): 1: handles elementary ops, 0: superinstruction-only
+                    // programs, 4: tape in global memory, 5: idem, CTA-wide teams
     coop_fn step, prop;
 };
 
