@@ -15,8 +15,10 @@
 //   * shared memory otherwise only holds what threads exchange: the positions of the current order pair and the
 //     outputs of the pair interactions / partial sums ([role][pair][lane] so that a warp writes consecutive slots);
 //   * what a thread does in the summation phase is a pre-decoded 32-byte record (nb_role) per round;
-//   * the three infinity norms of the step-size estimate are gathered while the coefficients are produced
-//     (shared-memory atomic max on the bit patterns of |x|): no second pass over the coefficients for h.
+//   * the three infinity norms of the step-size estimate are gathered while the coefficients are produced: no second
+//     pass over the coefficients for h. Warp teams of the 256-thread instantiations keep each thread's maxima in
+//     registers and reduce them with warp shuffles after the jet; the others use shared-memory atomic maxima on the
+//     bit patterns of |x|.
 // All shared-memory accesses use 32-bit shared-window addresses (ld.shared / st.shared): no generic addressing, no
 // 64-bit pointer arithmetic in the hot loops.
 // Replaces, for these programs: the JIT'd step function (src/taylor_00.cpp:712-865) and the propagate loop
@@ -60,6 +62,87 @@ struct nb_dev_plan {
     double *offchip;              // OFFCHIP kernels: per CTA, [order pair][3 rows][thread] pairs of doubles
     nb1_tab l1;                   // k_nb1 only
 };
+
+// Per-phase cycle attribution of k_nb (warp teams, PROP), compiled in with -DHY_NB_PHASE_CLOCK only
+// (tools/nb_phase_profile.py): thread 0 of every team adds the clock64() cycles between the phase boundaries to
+// nb_phase_cycles[team][phase], and counts the team's warp-steps and its lifetime. The sub-phases split the pair and
+// summation phases of thread 0 further: each ends where the instructions of its part have been issued, so the latency
+// of a load is charged to the sub-phase that first uses the value; what is left of a phase after its sub-phases is the
+// wait at the synchronisation that ends it. Without the macro the object has no state and emits no code.
+enum nb_phase : int {
+    NB_PH_PAIR,      // pair_block() of an order pair, and the sync after it
+    NB_PH_SUM,       // the summation rounds of an order pair and their syncs
+    NB_PH_INIT,      // role_init(): order 0 from the state, and the sync after it
+    NB_PH_STEP_SIZE, // nb_step_size() on the owner threads, and the sync after it
+    NB_PH_UPDATE,    // coop_update_state() and the reduction of its non-finite mask
+    NB_PH_PROP,      // the lane_prop bookkeeping, the loop test and chunk changes
+    NB_PH_STEPS,     // (count of warp-steps)
+    NB_PH_LIFE,      // (cycles from the first chunk claim to the end of the kernel)
+    // Sub-phases of NB_PH_PAIR (nb::pair_block):
+    NB_PH_PAIR_SS,   //   d_k and the sum_sq loop, the rows d_k and r^2 stored
+    NB_PH_PAIR_MAIN, //   the main loop (pow recurrence and products)
+    NB_PH_PAIR_Q,    //   the two quotients of the pow recurrence, r^alpha stored
+    NB_PH_PAIR_OUT,  //   the last terms of the products and the output stores
+    // Sub-phases of NB_PH_SUM (per round, nb::role_block):
+    NB_PH_SUM_ROLE,  //   the role record
+    NB_PH_SUM_LOAD,  //   the term loads
+    NB_PH_SUM_ARITH, //   the sum and the quotients
+    NB_PH_SUM_STORE, //   the coefficient / position / partial-sum stores and the round's sync
+    NB_PH_SLOTS
+};
+#if defined(HY_NB_PHASE_CLOCK)
+constexpr std::uint32_t nb_phase_teams = 4096u;
+namespace
+{
+__device__ unsigned long long nb_phase_cycles[nb_phase_teams][NB_PH_SLOTS];
+}
+struct nb_phase_clock {
+    unsigned long long *acc;
+    long long t, t0, ts;
+    __device__ __forceinline__ void start(std::size_t team, bool leader)
+    {
+        acc = leader && team < nb_phase_teams ? nb_phase_cycles[team] : nullptr;
+        ts = t0 = t = clock64();
+    }
+    __device__ __forceinline__ void lap(nb_phase ph)
+    {
+        const long long now = clock64();
+        if (acc != nullptr) {
+            atomicAdd(acc + ph, static_cast<unsigned long long>(now - t));
+        }
+        ts = t = now;
+    }
+    // A sub-phase: the cycles since the last lap() or sub().
+    __device__ __forceinline__ void sub(nb_phase ph)
+    {
+        const long long now = clock64();
+        if (acc != nullptr) {
+            atomicAdd(acc + ph, static_cast<unsigned long long>(now - ts));
+        }
+        ts = now;
+    }
+    __device__ __forceinline__ void step()
+    {
+        if (acc != nullptr) {
+            atomicAdd(acc + NB_PH_STEPS, 1ull);
+        }
+    }
+    __device__ __forceinline__ void finish()
+    {
+        if (acc != nullptr) {
+            atomicAdd(acc + NB_PH_LIFE, static_cast<unsigned long long>(clock64() - t0));
+        }
+    }
+};
+#else
+struct nb_phase_clock {
+    __device__ __forceinline__ void start(std::size_t, bool) {}
+    __device__ __forceinline__ void lap(nb_phase) {}
+    __device__ __forceinline__ void sub(nb_phase) {}
+    __device__ __forceinline__ void step() {}
+    __device__ __forceinline__ void finish() {}
+};
+#endif
 
 namespace nbk
 {
@@ -123,6 +206,13 @@ struct pair_mem {
     std::uint32_t fac_, fac_stride_b;
     double2 *grow; // OFFCHIP: this thread's element (0, 0)
     std::uint32_t flags; // bit 0: active (owns a pair), bits 1-3: n_k exists
+#if defined(HY_NB_PHASE_CLOCK)
+    nb_phase_clock *clk;
+    __device__ __forceinline__ void lap(int k) const
+    {
+        clk->sub(static_cast<nb_phase>(NB_PH_PAIR_SS + k));
+    }
+#endif
 
     __device__ __forceinline__ d2 gld(std::uint32_t op, std::uint32_t r) const
     {
@@ -242,12 +332,16 @@ struct pair_mem {
 
 // Storage policy of role_block() / role_init(): the thread's NL lanes start at lane l0 of the team's LT lanes (the
 // records' units already include l0).
-template <int NL>
+// REGN: the thread keeps its maxima of the step-size norms in registers (nrm), reduced over the team with warp
+// shuffles once the jet is done (norms_reduce); otherwise they go to the team's norm slots in shared memory by atomic
+// maxima, which sm_90 executes as compare-and-swap loops.
+template <int NL, bool REGN>
 struct role_mem {
     std::uint32_t pos_b, out_b;   // team bases
     std::uint32_t consts, rcp_;   // CTA tables
     std::uint32_t norms;          // team norms: [3][LT] u64 (|x^[0]|, |x^[p]|, |x^[p-1]|), + lane l0 of this thread
     std::uint32_t lt8;            // copies * LT * 8: stride between the three norms
+    mutable double nrm[3][NL];    // REGN: this thread's maxima (|x^[0]|, |x^[p]|, |x^[p-1]|) of its lanes
     const double *state0;         // D.state + first global lane of this thread (clamped)
     std::size_t n_batch;
     double *cbase;                // coefficient store + lane offset of lane 0 of this thread
@@ -256,6 +350,13 @@ struct role_mem {
     bool pub, track;
     bool lane_ok[NL];
     std::uint32_t ldelta; // offset (in doubles) between the thread's lanes in state / public store (0 if clamped)
+#if defined(HY_NB_PHASE_CLOCK)
+    nb_phase_clock *clk;
+    __device__ __forceinline__ void lap(int k) const
+    {
+        clk->sub(static_cast<nb_phase>(NB_PH_SUM_LOAD + k));
+    }
+#endif
 
     __device__ __forceinline__ d2 out_u(std::uint32_t unit, int l) const
     {
@@ -279,11 +380,64 @@ struct role_mem {
     }
     // Norms of the step-size estimate: NaN-skipping maximum of |v| (bit patterns of non-negative doubles order like
     // unsigned integers). which: 0 = order 0, 1 = order p, 2 = order p - 1.
+    // (REGN: fmax() skips the NaN and, on non-negative values, picks the same value as the maximum of the bit
+    // patterns, so the result is the same bits.)
     __device__ __forceinline__ void norm(std::uint32_t which, int l, double v) const
     {
-        if (v == v) {
+        if constexpr (REGN) {
+            // (Constant indices: a register, not a local-memory array.)
+            if (which == 0u) {
+                nrm[0][l] = fmax(nrm[0][l], fabs(v));
+            } else if (which == 1u) {
+                nrm[1][l] = fmax(nrm[1][l], fabs(v));
+            } else {
+                nrm[2][l] = fmax(nrm[2][l], fabs(v));
+            }
+        } else if (v == v) {
             red_max_u64(norms + which * lt8 + l * 8u,
                         static_cast<unsigned long long>(__double_as_longlong(v)) & 0x7fffffffffffffffull);
+        }
+    }
+    __device__ __forceinline__ void norms_reset() const
+    {
+        if constexpr (!REGN) {
+            return;
+        }
+#pragma unroll
+        for (int w = 0; w < 3; ++w) {
+#pragma unroll
+            for (int l = 0; l < NL; ++l) {
+                nrm[w][l] = 0.;
+            }
+        }
+    }
+    // REGN, warp teams of LT lanes: the maxima of lane tid (< LT) of the team, for its owner thread. Threads whose
+    // indices differ by a multiple of GS = LT / NL hold the same lanes: a butterfly over those strides gives each of
+    // them the team's maxima. Every thread of the warp takes part.
+    template <int LT>
+    __device__ __forceinline__ void norms_reduce(std::uint32_t tid, double (&m3)[3]) const
+    {
+        constexpr int GS = LT / NL;
+#pragma unroll
+        for (int off = GS; off < 32; off *= 2) {
+#pragma unroll
+            for (int w = 0; w < 3; ++w) {
+#pragma unroll
+                for (int l = 0; l < NL; ++l) {
+                    nrm[w][l] = fmax(nrm[w][l], __shfl_xor_sync(0xffffffffu, nrm[w][l], off));
+                }
+            }
+        }
+        // Lane tid is element tid % NL of the threads with thread index % GS == tid / NL.
+        const int src = static_cast<int>((tid % LT) / NL);
+#pragma unroll
+        for (int w = 0; w < 3; ++w) {
+            double v = __shfl_sync(0xffffffffu, nrm[w][0], src);
+            if constexpr (NL == 2) {
+                const double v1 = __shfl_sync(0xffffffffu, nrm[w][1], src);
+                v = (tid % 2u) != 0u ? v1 : v;
+            }
+            m3[w] = v;
         }
     }
     __device__ __forceinline__ void track_order(std::uint32_t order, const double (&a)[NL]) const
@@ -362,88 +516,32 @@ struct role_mem {
 // ignores every other NaN (src/taylor_00.cpp:102-273). Once per lane and step: out of line. (The program's constants
 // come as values: a reference to the kernel's program would park a copy of it in local memory, read back from L2 at
 // every step.)
+// norms == nullptr: the maxima come in m0, mp, mp1 (reduced in registers, role_mem::norms_reduce()).
 static __device__ __noinline__ double nb_step_size(double inv_p, double inv_pm1, double rhofac, unsigned long long *norms,
-                                                   std::uint32_t lt, const double *c, std::size_t off_p,
-                                                   std::size_t off_pm1, double max_delta_t)
+                                                   std::uint32_t lt, double m0, double mp, double mp1, const double *c,
+                                                   std::size_t off_p, std::size_t off_pm1, double max_delta_t)
 {
-    // norms[(which * copies + r) * lt]: the maximum over the copies, which are reset.
-    const std::uint32_t copies = detail::nb_norm_copies(lt);
-    unsigned long long n3[3];
-    for (std::uint32_t w = 0; w < 3u; ++w) {
-        unsigned long long v = 0ull;
-        for (std::uint32_t r = 0; r < copies; ++r) {
-            unsigned long long *q = norms + (w * copies + r) * lt;
-            v = *q > v ? *q : v;
-            *q = 0ull;
+    if (norms != nullptr) {
+        // norms[(which * copies + r) * lt]: the maximum over the copies, which are reset.
+        const std::uint32_t copies = detail::nb_norm_copies(lt);
+        unsigned long long n3[3];
+        for (std::uint32_t w = 0; w < 3u; ++w) {
+            unsigned long long v = 0ull;
+            for (std::uint32_t r = 0; r < copies; ++r) {
+                unsigned long long *q = norms + (w * copies + r) * lt;
+                v = *q > v ? *q : v;
+                *q = 0ull;
+            }
+            n3[w] = v;
         }
-        n3[w] = v;
+        m0 = __longlong_as_double(static_cast<long long>(n3[0]));
+        mp = __longlong_as_double(static_cast<long long>(n3[1]));
+        mp1 = __longlong_as_double(static_cast<long long>(n3[2]));
     }
-    const double m0 = __longlong_as_double(static_cast<long long>(n3[0]));
-    const double mp = __longlong_as_double(static_cast<long long>(n3[1]));
-    const double mp1 = __longlong_as_double(static_cast<long long>(n3[2]));
     const double f0 = fabs(c[0]), fp = fabs(c[off_p]), fp1 = fabs(c[off_pm1]);
     return h_from_norms(inv_p, inv_pm1, rhofac, isnan(f0) ? f0 : m0, isnan(fp) ? fp : mp, isnan(fp1) ? fp1 : mp1,
                         max_delta_t);
 }
-
-// Per-phase cycle attribution of k_nb (warp teams, PROP), compiled in with -DHY_NB_PHASE_CLOCK only
-// (tools/nb_phase_profile.py): thread 0 of every team adds the clock64() cycles between the phase boundaries to
-// nb_phase_cycles[team][phase], and counts the team's warp-steps and its lifetime. Without the macro the object has
-// no state and emits no code.
-enum nb_phase : int {
-    NB_PH_PAIR,      // pair_block() of an order pair, and the sync after it
-    NB_PH_SUM,       // the summation rounds of an order pair and their syncs
-    NB_PH_INIT,      // role_init(): order 0 from the state, and the sync after it
-    NB_PH_STEP_SIZE, // nb_step_size() on the owner threads, and the sync after it
-    NB_PH_UPDATE,    // coop_update_state() and the reduction of its non-finite mask
-    NB_PH_PROP,      // the lane_prop bookkeeping, the loop test and chunk changes
-    NB_PH_STEPS,     // (count of warp-steps)
-    NB_PH_LIFE,      // (cycles from the first chunk claim to the end of the kernel)
-    NB_PH_SLOTS
-};
-#if defined(HY_NB_PHASE_CLOCK)
-constexpr std::uint32_t nb_phase_teams = 4096u;
-namespace
-{
-__device__ unsigned long long nb_phase_cycles[nb_phase_teams][NB_PH_SLOTS];
-}
-struct nb_phase_clock {
-    unsigned long long *acc;
-    long long t, t0;
-    __device__ __forceinline__ void start(std::size_t team, bool leader)
-    {
-        acc = leader && team < nb_phase_teams ? nb_phase_cycles[team] : nullptr;
-        t0 = t = clock64();
-    }
-    __device__ __forceinline__ void lap(nb_phase ph)
-    {
-        const long long now = clock64();
-        if (acc != nullptr) {
-            atomicAdd(acc + ph, static_cast<unsigned long long>(now - t));
-        }
-        t = now;
-    }
-    __device__ __forceinline__ void step()
-    {
-        if (acc != nullptr) {
-            atomicAdd(acc + NB_PH_STEPS, 1ull);
-        }
-    }
-    __device__ __forceinline__ void finish()
-    {
-        if (acc != nullptr) {
-            atomicAdd(acc + NB_PH_LIFE, static_cast<unsigned long long>(clock64() - t0));
-        }
-    }
-};
-#else
-struct nb_phase_clock {
-    __device__ __forceinline__ void start(std::size_t, bool) {}
-    __device__ __forceinline__ void lap(nb_phase) {}
-    __device__ __forceinline__ void step() {}
-    __device__ __forceinline__ void finish() {}
-};
-#endif
 
 // LT: lanes per team; CTA: a team is the whole CTA (else a warp); OFFCHIP: r^2, d_2, r^alpha rows in NP.offchip.
 template <int LT, bool CTA, bool OFFCHIP, bool PROP, int MAXT>
@@ -540,7 +638,9 @@ __global__ void __launch_bounds__(MAXT, 1) k_nb(program P, nb_dev_plan NP, batch
     }
     // ---- this thread's lanes in the summation phase ----
     const std::uint32_t l0 = (tid % GS) * NL;
-    nbk::role_mem<NL> RM;
+    // (The 384- and 512-thread instantiations have no registers to spare for the maxima.)
+    constexpr bool REGN = !CTA && MAXT <= 256;
+    nbk::role_mem<NL, REGN> RM;
     RM.pos_b = pos_b;
     RM.out_b = out_b;
     RM.consts = nbk::saddr(consts_s);
@@ -568,6 +668,10 @@ __global__ void __launch_bounds__(MAXT, 1) k_nb(program P, nb_dev_plan NP, batch
     const bool owner = tid < LT;
     const std::uint32_t n_blocks = NP.npp;
     nb_phase_clock clk;
+#if defined(HY_NB_PHASE_CLOCK)
+    PM.clk = &clk;
+    RM.clk = &clk;
+#endif
 
     const auto load_role = [&](std::uint32_t rd, std::uint32_t (&w)[8]) {
         uint4 a, b;
@@ -581,6 +685,7 @@ __global__ void __launch_bounds__(MAXT, 1) k_nb(program P, nb_dev_plan NP, batch
         w[0] = a.x, w[1] = a.y, w[2] = a.z, w[3] = a.w, w[4] = b.x, w[5] = b.y, w[6] = b.z, w[7] = b.w;
     };
 
+    double nm3[3] = {0., 0., 0.}; // REGN: the maxima of the owner's lane after a jet
     const auto jet = [&](std::uint32_t lane0) {
         // The thread's lanes: global indices (clamped), offsets into the coefficient store.
         {
@@ -596,6 +701,7 @@ __global__ void __launch_bounds__(MAXT, 1) k_nb(program P, nb_dev_plan NP, batch
             RM.cbase = cv.base + cv.lane_off(ga, l0);
         }
         RM.track = true;
+        RM.norms_reset();
         for (std::uint32_t rd = 0; rd < n_rounds; ++rd) {
             std::uint32_t w[8];
             load_role(rd, w);
@@ -613,20 +719,25 @@ __global__ void __launch_bounds__(MAXT, 1) k_nb(program P, nb_dev_plan NP, batch
             for (std::uint32_t rd = 0; rd < n_rounds; ++rd) {
                 std::uint32_t w[8];
                 load_role(rd, w);
+                clk.sub(NB_PH_SUM_ROLE);
                 nb::role_block<NL>(RM, w, m, p);
                 if (((level_end >> rd) & 1u) != 0u) {
                     T::sync();
                 }
+                clk.sub(NB_PH_SUM_STORE);
             }
             clk.lap(NB_PH_SUM);
+        }
+        if constexpr (REGN) {
+            RM.template norms_reduce<LT>(tid, nm3);
         }
     };
 
     // Step size from the norms gathered during the jet (owner threads: one lane each); resets the norms.
     const auto step_size = [&](std::uint32_t lane, double max_delta_t) {
         const double *c = cv.base + cv.lane_off(lane, tid);
-        return nb_step_size(P.inv_p, P.inv_pm1, P.rhofac, norms_p + tid, LT, c, p * cv.stride_o, (p - 1u) * cv.stride_o,
-                            max_delta_t);
+        return nb_step_size(P.inv_p, P.inv_pm1, P.rhofac, REGN ? nullptr : norms_p + tid, LT, nm3[0], nm3[1], nm3[2], c,
+                            p * cv.stride_o, (p - 1u) * cv.stride_o, max_delta_t);
     };
     if (owner) {
         for (std::uint32_t i = 0; i < 3u * NC; ++i) {
