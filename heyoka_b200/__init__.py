@@ -7,6 +7,7 @@ reference's own tests (test/taylor_adaptive_batch.cpp). The product is the nativ
 Python or CPU fallback for the compute path: if the library is missing, importing fails loudly.
 """
 import ctypes as C
+import enum
 import os
 
 import numpy as np
@@ -16,7 +17,7 @@ from ._capi import lib, check, HyError  # noqa: F401
 
 __all__ = [
     "expression", "make_vars", "par", "time", "sin", "cos", "tanh", "exp", "log", "sigmoid", "relu", "relup", "sqrt", "square", "pow", "sum",
-    "prod", "model", "taylor_adaptive_batch", "t_event_batch", "nt_event_batch", "event_direction", "continuous_output_batch", "taylor_outcome", "Program", "Batch", "order_from_tol", "HyError",
+    "prod", "diff", "var_args", "var_ode_sys", "model", "taylor_adaptive_batch", "t_event_batch", "nt_event_batch", "event_direction", "continuous_output_batch", "taylor_outcome", "Program", "Batch", "order_from_tol", "HyError",
 ]
 
 
@@ -173,6 +174,49 @@ def prod(terms):
     return _func("prod", *terms)
 
 
+def diff(e, wrt):
+    """Symbolic derivative of e with respect to a variable or a parameter par[i] (folded like every builder)."""
+    e, wrt = expression._wrap(e), expression._wrap(wrt)
+    return expression(_handle=_capi.ex_checked(lib.hy_ex_diff(e._h, wrt._h)))
+
+
+class var_args(enum.IntFlag):
+    """Arguments of the variational equations: the state variables (LHS order), the parameters (index order), the
+    initial time (not implemented). vars | params: the state variables first."""
+    vars = 1
+    params = 2
+    time = 4
+    all = 7
+
+
+class var_ode_sys:
+    """An ODE system augmented with its first-order variational equations (heyoka_b200/var_ode_sys.hpp).
+
+    args: var_args flags, or a list of state variables and / or parameters, kept in the order given. The augmented
+    state is [x_0 .. x_{n-1}, dx_0/da_0 .. dx_0/da_{m-1}, dx_1/da_0, ...]: state[n:] reshaped to (n, m) is the STM."""
+
+    def __init__(self, sys, args=var_args.vars, order=1):
+        keep = [(expression._wrap(lhs), expression._wrap(rhs)) for lhs, rhs in sys]
+        n = len(keep)
+        lhs = (C.c_void_p * max(n, 1))(*[p[0]._h for p in keep])
+        rhs = (C.c_void_p * max(n, 1))(*[p[1]._h for p in keep])
+        if isinstance(args, int):
+            flags, items = int(args), []  # (no flags: an empty explicit list, refused by the native code)
+        else:
+            flags, items = 0, [expression._wrap(a) for a in args]
+        arr = (C.c_void_p * max(len(items), 1))(*[a._h for a in items])
+        n_eq, n_args = C.c_uint32(), C.c_uint32()
+        call = lambda ol, orr, oa: lib.hy_var_ode_sys(lhs, rhs, n, flags, arr, len(items), int(order),  # noqa: E731
+                                                      C.byref(n_eq), C.byref(n_args), ol, orr, oa)
+        check(call(None, None, None))
+        ol, orr, oa = (C.c_void_p * n_eq.value)(), (C.c_void_p * n_eq.value)(), (C.c_void_p * n_args.value)()
+        check(call(ol, orr, oa))
+        self.sys = [(expression(_handle=ol[i]), expression(_handle=orr[i])) for i in range(n_eq.value)]
+        self.vargs = [expression(_handle=oa[j]) for j in range(n_args.value)]
+        self.n_orig_sv = n
+        self.order = int(order)
+
+
 class model:
     """model::nbody / pendulum / ffnn (src/model/*.cpp)."""
 
@@ -229,6 +273,8 @@ class Program:
         if _handle is not None:
             self._h = _handle
         else:
+            if isinstance(sys, var_ode_sys):
+                sys = sys.sys  # (the augmented system is an ordinary ODE system for the stepper)
             n = len(sys)
             self._keep = [(expression._wrap(lhs), expression._wrap(rhs)) for lhs, rhs in sys]
             self._keep_ev = [expression._wrap(e) for e in events]
@@ -459,6 +505,20 @@ class Batch:
         check(lib.hy_batch_d_output(self._h, _dptr(tau), _dptr(out)))
         return out
 
+    def eval_taylor_map(self, n_orig_sv, dx, out=None):
+        """Taylor map x + Phi dx of the resident state (hy_batch_eval_taylor_map()): dx [n_args, batch] on the host,
+        returns out [n_orig_sv, batch]."""
+        dx = np.ascontiguousarray(dx, dtype=np.float64).reshape(-1, self.n)
+        out = np.empty((n_orig_sv, self.n)) if out is None else out
+        assert out.dtype == np.float64 and out.flags["C_CONTIGUOUS"] and out.size == n_orig_sv * self.n
+        check(lib.hy_batch_eval_taylor_map(self._h, int(n_orig_sv), dx.shape[0], _dptr(dx), _dptr(out), 0))
+        return out
+
+    def eval_taylor_map_dev(self, n_orig_sv, n_args, d_dx, d_out):
+        """The same on device pointers (ints, e.g. torch data_ptr()), enqueued on the batch's stream."""
+        vp = lambda x: C.cast(C.c_void_p(int(x)), C.POINTER(C.c_double))  # noqa: E731
+        check(lib.hy_batch_eval_taylor_map(self._h, int(n_orig_sv), int(n_args), vp(d_dx), vp(d_out), 1))
+
     # --- events (include/heyoka_b200.h, section E) ---
     def set_events(self, n_te, dirs, cooldowns, tol):
         d = np.ascontiguousarray(dirs, dtype=np.int32)
@@ -597,10 +657,14 @@ class taylor_adaptive_batch:
             raise ValueError("The batch size in an adaptive Taylor integrator cannot be zero")
         self._tes, self._ntes = list(t_events or []), list(nt_events or [])
         self._with_events = bool(self._tes or self._ntes)
+        self._vsys = sys if isinstance(sys, var_ode_sys) else None
         self._prog = Program(sys, tol=tol, high_accuracy=high_accuracy,
                              events=[e.ex for e in self._tes] + [e.ex for e in self._ntes])
         P = self._prog
         state = np.array(state, dtype=np.float64)
+        if self._vsys is not None and state.size in (0, self._vsys.n_orig_sv * batch_size):
+            state = _var_initial_state(self._vsys, state, batch_size)
+        self._tstate = None if self._vsys is None else np.zeros((self._vsys.n_orig_sv, batch_size))
         # Size checks of finalise_ctor_impl(), src/taylor_adaptive_batch.cpp:164-274.
         if state.size != P.n_eq * batch_size:
             raise ValueError(
@@ -732,6 +796,71 @@ class taylor_adaptive_batch:
 
     def get_decomposition_str(self):
         return self._prog.dc_str()
+
+    # --- variational integrators (constructed from a var_ode_sys) ---------------------------------
+    @property
+    def is_variational(self):
+        return self._vsys is not None
+
+    @property
+    def n_orig_sv(self):
+        return self._prog.n_eq if self._vsys is None else self._vsys.n_orig_sv
+
+    @property
+    def vorder(self):
+        return 0 if self._vsys is None else self._vsys.order
+
+    @property
+    def vargs(self):
+        return [] if self._vsys is None else list(self._vsys.vargs)
+
+    def _check_variational(self, what):
+        if self._vsys is None:
+            raise ValueError("The function %s can be invoked only on a variational integrator" % what)
+
+    def get_vslice(self, order, component=None):
+        """Rows of the state holding the derivatives of the given order (0: the original state variables), of all
+        components or of one."""
+        self._check_variational("get_vslice()")
+        n, m = self._vsys.n_orig_sv, len(self._vsys.vargs)
+        if order > self._vsys.order:
+            raise ValueError("Cannot fetch the slice of the derivatives of order %d in a variational integrator of "
+                             "order %d" % (order, self._vsys.order))
+        if component is None:
+            return slice(0, n) if order == 0 else slice(n, n * (1 + m))
+        if not 0 <= component < n:
+            raise ValueError("Cannot fetch the slice of the derivatives of the component %d in a variational "
+                             "integrator with %d original state variables" % (component, n))
+        return slice(component, component + 1) if order == 0 else slice(n + component * m, n + (component + 1) * m)
+
+    def get_mindex(self, i):
+        """Dense multi-index of state row i: [component, n_0, .., n_{m-1}]."""
+        self._check_variational("get_mindex()")
+        n, m = self._vsys.n_orig_sv, len(self._vsys.vargs)
+        if not 0 <= i < n * (1 + m):
+            raise ValueError("Cannot fetch the multi-index of the state variable %d in a variational integrator with "
+                             "%d state variables" % (i, n * (1 + m)))
+        if i < n:
+            return [i] + [0] * m
+        k = i - n
+        return [k // m] + [1 if j == k % m else 0 for j in range(m)]
+
+    def eval_taylor_map(self, dx):
+        """Taylor map x + Phi dx of the current state, on the device: dx [n_args, batch]; returns tstate
+        [n_orig_sv, batch]."""
+        self._check_variational("eval_taylor_map()")
+        m, n = len(self._vsys.vargs), self._batch_size
+        dx = np.asarray(dx, dtype=np.float64)
+        if dx.size != m * n:
+            raise ValueError("Invalid number of values passed to eval_taylor_map(): %d values were passed, but %d are "
+                             "needed (%d arguments in batches of %d)" % (dx.size, m * n, m, n))
+        self._push()
+        self._b.eval_taylor_map(self._vsys.n_orig_sv, dx.reshape(m, n), out=self._tstate)
+        return self._tstate
+
+    @property
+    def tstate(self):
+        return self._tstate
 
     # --- stepping ------------------------------------------------------------------------------
     def _push(self):
@@ -1146,6 +1275,20 @@ class taylor_adaptive_batch:
             hi, lo = _dfloat_add(self._t_hi, self._t_lo, -self._last_h, np.zeros(n))
             tau, _ = _dfloat_add(t, np.zeros(n), -hi, -lo)
         return self._b.d_output(tau)
+
+
+def _var_initial_state(vsys, state, batch):
+    """The constructor's fill of the variational rows (taylor.hpp): original rows as given (zeros if the state is
+    empty); per lane, the STM column of an argument that is the state variable x_k is e_k, that of a parameter 0."""
+    n, m = vsys.n_orig_sv, len(vsys.vargs)
+    full = np.zeros((n * (1 + m), batch))
+    if state.size:
+        full[:n] = state.reshape(n, batch)
+    for i in range(n):
+        for j, a in enumerate(vsys.vargs):
+            if repr(diff(a, vsys.sys[i][0])) == "1":  # a is the state variable x_i (a parameter gives 0)
+                full[n + i * m + j] = 1.0
+    return full
 
 
 def _eft_knuth(a, b):

@@ -78,6 +78,9 @@ SIGNATURES = {
     "hy_ex_copy": (_vp, [_vp]),
     "hy_ex_free": (None, [_vp]),
     "hy_ex_str": (C.c_size_t, [_vp, C.c_char_p, C.c_size_t]),
+    "hy_ex_diff": (_vp, [_vp, _vp]),
+    "hy_var_ode_sys": (C.c_int, [_vpp, _vpp, C.c_uint32, C.c_uint32, _vpp, C.c_uint32, C.c_uint32,
+                                 C.POINTER(C.c_uint32), C.POINTER(C.c_uint32), _vpp, _vpp, _vpp]),
     "hy_model_nbody": (C.c_int, [C.c_uint32, _dp, C.c_uint32, C.c_double, _vpp, _vpp]),
     "hy_model_pendulum": (C.c_int, [C.c_double, C.c_double, _vpp, _vpp]),
     "hy_model_ffnn": (C.c_int, [_vpp, C.c_uint32, C.POINTER(C.c_uint32), C.c_uint32, C.c_uint32, C.POINTER(C.c_int), _dp,
@@ -127,6 +130,7 @@ SIGNATURES = {
     "hy_cout_download": (C.c_int, [_vp, _dp, _dp, _dp]),
     "hy_cout_destroy": (None, [_vp]),
     "hy_batch_d_output": (C.c_int, [_vp, _dp, _dp]),
+    "hy_batch_eval_taylor_map": (C.c_int, [_vp, C.c_uint32, C.c_uint32, _dp, _dp, C.c_int]),
     "hy_batch_set_events": (C.c_int, [_vp, C.c_uint32, C.POINTER(C.c_int32), _dp, C.c_double]),
     "hy_batch_n_events": (C.c_uint32, [_vp]),
     "hy_batch_get_events": (C.c_int, [_vp, C.POINTER(hy_event_rec), C.c_uint32]),

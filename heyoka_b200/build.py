@@ -18,7 +18,7 @@ OBJDIR = os.path.join(ROOT, "build", "obj")
 LIB = os.path.join(LIBDIR, "libheyoka_b200.so")
 
 HOST_SOURCES = ["expression.cpp", "decompose.cpp", "model.cpp", "lower.cpp", "smem_plan.cpp", "nb_plan.cpp", "nn_plan.cpp",
-                "capi_host.cpp", "taylor_adaptive_batch.cpp"]
+                "capi_host.cpp", "taylor_adaptive_batch.cpp", "var_ode_sys.cpp"]
 CUDA_SOURCES = ["batch.cu", "nn_inst.cu", "nb1_inst.cu"]
 # The cooperative kernel is instantiated per (lanes per thread, max threads per CTA, mode) family, one
 # object each (built in parallel).

@@ -295,6 +295,8 @@ struct hy_batch {
     std::size_t slab_doubles = 0; // one warp's tape slab of k_hbm
     double *d_tmp = nullptr;      // 3 * n doubles: staged per-lane inputs (t_final hi/lo, max_delta_t)
     double *d_snapshot = nullptr; // state + time snapshot for the global-exit replay
+    double *d_tmap = nullptr;     // staged dx and out of hy_batch_eval_taylor_map() (host form), allocated on first use
+    std::size_t tmap_doubles = 0;
     unsigned int *d_counter = nullptr;
     dev::run_flags *d_flags = nullptr;
 
@@ -362,7 +364,8 @@ void hy_batch::free_all() noexcept
           static_cast<void *>(d_tmp),
           static_cast<void *>(d_snapshot), static_cast<void *>(d_counter), static_cast<void *>(d_flags),
           static_cast<void *>(d_nb_pairs), static_cast<void *>(d_nb_roles), static_cast<void *>(d_nb_consts),
-          static_cast<void *>(d_nb_fac), static_cast<void *>(d_nn_wimg), static_cast<void *>(d_nn_out)}) {
+          static_cast<void *>(d_nb_fac), static_cast<void *>(d_nn_wimg), static_cast<void *>(d_nn_out),
+          static_cast<void *>(d_tmap)}) {
         if (p != nullptr) {
             cudaFree(p);
         }
@@ -3021,6 +3024,83 @@ int hy_batch_d_output(hy_batch *b, const double *tau, double *out)
                                           b->stream));
         }
         HY_CUDA_CHECK(cudaStreamSynchronize(b->stream));
+        return HY_OK;
+    } catch (...) {
+        return translate_exception();
+    }
+}
+
+namespace
+{
+
+// k_taylor_map on one single-device batch, device-resident dx / out.
+void taylor_map_launch(hy_batch *b, std::uint32_t n_orig, std::uint32_t m, const double *d_dx, double *d_out)
+{
+    const std::uint32_t chunk = std::min(m, dev::TMAP_CHUNK);
+    dev::k_taylor_map<<<(b->n + dev::TMAP_THREADS - 1u) / dev::TMAP_THREADS, dev::TMAP_THREADS,
+                        sizeof(double) * chunk * dev::TMAP_THREADS, b->stream>>>(b->d_state, b->n, n_orig, m, d_dx,
+                                                                                 d_out);
+    HY_CUDA_CHECK(cudaGetLastError());
+    ++b->n_launches;
+}
+
+// Host form: dx staged into d_tmap[0, m * n), the result read back from d_tmap[m * n, (m + n_orig) * n).
+void taylor_map_host(hy_batch *b, std::uint32_t n_orig, std::uint32_t m, const double *dx, double *out,
+                     std::size_t pitch, std::size_t off)
+{
+    const std::size_t need = static_cast<std::size_t>(m + n_orig) * b->n;
+    if (b->tmap_doubles < need) {
+        if (b->d_tmap != nullptr) {
+            HY_CUDA_CHECK(cudaStreamSynchronize(b->stream));
+            HY_CUDA_CHECK(cudaFree(b->d_tmap));
+            b->d_tmap = nullptr;
+            b->tmap_doubles = 0;
+        }
+        b->d_tmap = b->dalloc<double>(need);
+        b->tmap_doubles = need;
+    }
+    double *d_dx = b->d_tmap, *d_out = b->d_tmap + static_cast<std::size_t>(m) * b->n;
+    rows_h2d(b, d_dx, dx, m, pitch, off);
+    taylor_map_launch(b, n_orig, m, d_dx, d_out);
+    rows_d2h(b, out, d_out, n_orig, pitch, off);
+    HY_CUDA_CHECK(cudaStreamSynchronize(b->stream));
+}
+
+} // namespace
+
+int hy_batch_eval_taylor_map(hy_batch *b, uint32_t n_orig_sv, uint32_t n_args, const double *dx, double *out,
+                             int on_device)
+{
+    try {
+        if (b == nullptr || dx == nullptr || out == nullptr) {
+            throw std::invalid_argument("Null pointer passed to hy_batch_eval_taylor_map()");
+        }
+        if (n_orig_sv == 0u || n_args == 0u
+            || static_cast<std::uint64_t>(n_orig_sv) * (1u + static_cast<std::uint64_t>(n_args)) != b->n_eq) {
+            throw std::invalid_argument(
+                "Invalid sizes passed to hy_batch_eval_taylor_map(): " + std::to_string(n_orig_sv)
+                + " original state variables and " + std::to_string(n_args)
+                + " arguments do not make a variational system of order 1 with " + std::to_string(b->n_eq)
+                + " equations");
+        }
+        if (!b->shards.empty()) {
+            if (on_device) {
+                throw std::invalid_argument(
+                    "Device-resident arrays are not available for the Taylor map of a multi-device batch");
+            }
+            // Every shard evaluates its own lanes on its own device.
+            for_each_shard(b, [&](hy_batch *sh, std::size_t i) {
+                taylor_map_host(sh, n_orig_sv, n_args, dx, out, b->n, b->shard_off[i]);
+            });
+            return HY_OK;
+        }
+        device_guard guard(b->device);
+        if (on_device) {
+            // (Asynchronous on the batch's stream, like the other device-resident entry points.)
+            taylor_map_launch(b, n_orig_sv, n_args, dx, out);
+        } else {
+            taylor_map_host(b, n_orig_sv, n_args, dx, out, b->n, 0);
+        }
         return HY_OK;
     } catch (...) {
         return translate_exception();

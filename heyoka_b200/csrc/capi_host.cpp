@@ -14,6 +14,7 @@
 #include <heyoka_b200/expression.hpp>
 #include <heyoka_b200/model.hpp>
 #include <heyoka_b200/taylor_decompose.hpp>
+#include <heyoka_b200/var_ode_sys.hpp>
 
 #include "capi_common.hpp"
 #include "program.hpp"
@@ -39,6 +40,9 @@ int translate_exception()
     try {
         throw;
     } catch (const not_implemented_error &e) {
+        set_last_error(e.what());
+        return HY_ERR_NOT_IMPLEMENTED;
+    } catch (const hy::not_implemented_error &e) {
         set_last_error(e.what());
         return HY_ERR_NOT_IMPLEMENTED;
     } catch (const cuda_error &e) {
@@ -236,6 +240,67 @@ size_t hy_ex_str(const hy_ex *e, char *buf, size_t buf_len)
         return copy_out("", buf, buf_len);
     }
     return copy_out(hy::to_string(e->ex), buf, buf_len);
+}
+
+hy_ex *hy_ex_diff(const hy_ex *e, const hy_ex *wrt)
+{
+    return make_ex([&] {
+        if (e == nullptr || wrt == nullptr) {
+            throw std::invalid_argument("Null expression handle");
+        }
+        return hy::diff(e->ex, wrt->ex);
+    });
+}
+
+int hy_var_ode_sys(const hy_ex *const *lhs, const hy_ex *const *rhs, uint32_t n_eq, uint32_t flags,
+                   const hy_ex *const *args, uint32_t n_args, uint32_t order, uint32_t *n_out_eq, uint32_t *n_out_args,
+                   hy_ex **out_lhs, hy_ex **out_rhs, hy_ex **out_args)
+{
+    try {
+        if ((n_eq != 0u && (lhs == nullptr || rhs == nullptr)) || n_out_eq == nullptr || n_out_args == nullptr
+            || (flags == 0u && n_args != 0u && args == nullptr)) {
+            throw std::invalid_argument("Null pointer passed to hy_var_ode_sys()");
+        }
+        std::vector<std::pair<hy::expression, hy::expression>> sys;
+        for (uint32_t i = 0; i < n_eq; ++i) {
+            if (lhs[i] == nullptr || rhs[i] == nullptr) {
+                throw std::invalid_argument("Null expression handle");
+            }
+            sys.emplace_back(lhs[i]->ex, rhs[i]->ex);
+        }
+        std::variant<hy::var_args, std::vector<hy::expression>> va;
+        if (flags != 0u) {
+            if ((flags & ~(HY_VAR_ARGS_VARS | HY_VAR_ARGS_PARAMS | HY_VAR_ARGS_TIME)) != 0u) {
+                throw std::invalid_argument("Invalid flags passed to hy_var_ode_sys(): " + std::to_string(flags));
+            }
+            va = static_cast<hy::var_args>(flags);
+        } else {
+            std::vector<hy::expression> v;
+            for (uint32_t i = 0; i < n_args; ++i) {
+                if (args[i] == nullptr) {
+                    throw std::invalid_argument("Null expression handle");
+                }
+                v.push_back(args[i]->ex);
+            }
+            va = std::move(v);
+        }
+        const hy::var_ode_sys vsys(sys, va, order);
+        const auto &aug = vsys.get_sys();
+        *n_out_eq = static_cast<uint32_t>(aug.size());
+        *n_out_args = static_cast<uint32_t>(vsys.get_vargs().size());
+        if (out_lhs != nullptr && out_rhs != nullptr && out_args != nullptr) {
+            for (std::size_t i = 0; i < aug.size(); ++i) {
+                out_lhs[i] = new hy_ex{aug[i].first};
+                out_rhs[i] = new hy_ex{aug[i].second};
+            }
+            for (std::size_t j = 0; j < vsys.get_vargs().size(); ++j) {
+                out_args[j] = new hy_ex{vsys.get_vargs()[j]};
+            }
+        }
+        return HY_OK;
+    } catch (...) {
+        return translate_exception();
+    }
 }
 
 int hy_model_nbody(uint32_t n, const double *masses, uint32_t n_masses, double G, hy_ex **lhs, hy_ex **rhs)

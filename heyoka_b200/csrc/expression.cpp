@@ -7,6 +7,7 @@
 #include <set>
 #include <sstream>
 #include <stdexcept>
+#include <unordered_map>
 #include <unordered_set>
 
 namespace heyoka_b200
@@ -552,6 +553,130 @@ bool is_time_dependent(const std::vector<expression> &v)
         }
     }
     return false;
+}
+
+// ---------------------------------------------------------------------------------------------
+// Symbolic differentiation. One rule per func_kind a user expression can contain; shared subexpressions are
+// differentiated once (cache on function identity).
+// ---------------------------------------------------------------------------------------------
+namespace
+{
+
+bool is_zero(const expression &e)
+{
+    return e.is_number() && e.num() == 0.;
+}
+
+struct differ {
+    const expression &wrt;
+    std::unordered_map<const void *, expression> cache;
+
+    expression operator()(const expression &e)
+    {
+        switch (e.value().index()) {
+            case 0:
+                return expression{0.};
+            case 1:
+                return expression{wrt.is_variable() && wrt.var_name() == e.var_name() ? 1. : 0.};
+            case 2:
+                return expression{wrt.is_param() && wrt.par_idx() == e.par_idx() ? 1. : 0.};
+            default:
+                break;
+        }
+        if (const auto it = cache.find(e.fn_id()); it != cache.end()) {
+            return it->second;
+        }
+        auto ret = func_rule(e);
+        cache.emplace(e.fn_id(), ret);
+        return ret;
+    }
+
+    expression func_rule(const expression &e)
+    {
+        const auto &f = e.fn();
+        const auto chain = [&](expression outer) {
+            auto d = (*this)(f.args[0]);
+            return is_zero(d) ? expression{0.} : prod({std::move(outer), std::move(d)});
+        };
+        switch (f.kind) {
+            case func_kind::sum: {
+                std::vector<expression> terms;
+                for (const auto &a : f.args) {
+                    terms.push_back((*this)(a));
+                }
+                return sum(std::move(terms));
+            }
+            case func_kind::prod: {
+                // Product rule over all factors: sum_i (prod_{k != i} a_k) * a_i'.
+                std::vector<expression> terms;
+                for (std::size_t i = 0; i < f.args.size(); ++i) {
+                    auto d = (*this)(f.args[i]);
+                    if (is_zero(d)) {
+                        continue;
+                    }
+                    auto factors = f.args;
+                    factors[i] = std::move(d);
+                    terms.push_back(prod(std::move(factors)));
+                }
+                return sum(std::move(terms));
+            }
+            case func_kind::pow: {
+                const auto &x = f.args[0], &ex = f.args[1];
+                std::vector<expression> terms;
+                auto dx = (*this)(x);
+                if (!is_zero(dx)) {
+                    auto em1 = ex.is_number() ? expression{ex.num() - 1.} : sum({ex, expression{-1.}});
+                    terms.push_back(prod({ex, pow(x, em1), std::move(dx)}));
+                }
+                if (!ex.is_number()) {
+                    auto de = (*this)(ex);
+                    if (!is_zero(de)) {
+                        terms.push_back(prod({e, log(x), std::move(de)}));
+                    }
+                }
+                return sum(std::move(terms));
+            }
+            case func_kind::sin:
+                return chain(cos(f.args[0]));
+            case func_kind::cos:
+                return chain(prod({expression{-1.}, sin(f.args[0])}));
+            case func_kind::tanh:
+                // 1 - tanh(x)^2.
+                return chain(sum({expression{1.}, prod({expression{-1.}, pow(e, expression{2.})})}));
+            case func_kind::exp:
+                return chain(e);
+            case func_kind::log:
+                return chain(pow(f.args[0], expression{-1.}));
+            case func_kind::sigmoid:
+                // sigmoid(x) * (1 - sigmoid(x)).
+                return chain(prod({e, sum({expression{1.}, prod({expression{-1.}, e})})}));
+            case func_kind::relu:
+                // The leaky ReLU's derivative keeps its slope.
+                return chain(relup(f.args[0], f.args[1].num()));
+            case func_kind::relup:
+            case func_kind::time:
+                return expression{0.};
+            case func_kind::sub:
+            case func_kind::div:
+            case func_kind::sum_sq:
+            case func_kind::num_identity:
+                break;
+        }
+        throw std::invalid_argument(std::string("Cannot differentiate the function '") + func_kind_name(f.kind)
+                                    + "': it is created by the Taylor decomposition only");
+    }
+};
+
+} // namespace
+
+expression diff(const expression &e, const expression &wrt)
+{
+    if (!wrt.is_variable() && !wrt.is_param()) {
+        throw std::invalid_argument("Derivatives can be taken only with respect to a variable or a parameter, not "
+                                    "with respect to '"
+                                    + to_string(wrt) + "'");
+    }
+    return differ{wrt, {}}(e);
 }
 
 } // namespace heyoka_b200

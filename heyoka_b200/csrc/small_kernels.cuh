@@ -319,6 +319,43 @@ __global__ void k_selftest_div(unsigned long long n, unsigned long long seed, un
     }
 }
 
+// Taylor map of a variational batch of order 1 (hy_batch_eval_taylor_map()): out_i = x_i + sum_j Phi_ij dx_j, with
+// x = state rows [0, n_orig) and Phi_ij = state row n_orig + i * m + j. One thread per lane, lanes the coalesced axis.
+// Fixed arithmetic, so that a sequential restatement gives the same bits: acc = x_i, then for j = 0 .. m - 1
+// acc = acc + Phi_ij * dx_j with the product and the sum each rounded to nearest (__dmul_rn / __dadd_rn: no
+// contraction). The kernel streams Phi once: dx is loaded once per lane into shared memory (a per-thread column, so no
+// barrier is needed) in chunks of at most TMAP_CHUNK arguments and reused across the n_orig rows; with more arguments
+// than one chunk the partial sums go through `out` between chunks, which keeps the order of the additions.
+constexpr std::uint32_t TMAP_THREADS = 128, TMAP_CHUNK = 40;
+
+__global__ void __launch_bounds__(TMAP_THREADS) k_taylor_map(const double *__restrict__ state, std::uint32_t n,
+                                                             std::uint32_t n_orig, std::uint32_t m,
+                                                             const double *__restrict__ dx, double *__restrict__ out)
+{
+    extern __shared__ double s_dx[]; // [chunk][TMAP_THREADS]
+    const std::uint32_t lane = blockIdx.x * TMAP_THREADS + threadIdx.x;
+    if (lane >= n) {
+        return;
+    }
+    const std::size_t N = n;
+    double *my_dx = s_dx + threadIdx.x;
+    for (std::uint32_t j0 = 0; j0 < m; j0 += TMAP_CHUNK) {
+        const std::uint32_t jn = min(TMAP_CHUNK, m - j0);
+        for (std::uint32_t j = 0; j < jn; ++j) {
+            my_dx[j * TMAP_THREADS] = dx[(j0 + j) * N + lane];
+        }
+        for (std::uint32_t i = 0; i < n_orig; ++i) {
+            const double *phi = state + (n_orig + static_cast<std::size_t>(i) * m + j0) * N + lane;
+            double acc = j0 == 0u ? state[i * N + lane] : out[i * N + lane];
+#pragma unroll 8
+            for (std::uint32_t j = 0; j < jn; ++j) {
+                acc = __dadd_rn(acc, __dmul_rn(__ldcs(phi + j * N), my_dx[j * TMAP_THREADS]));
+            }
+            out[i * N + lane] = acc;
+        }
+    }
+}
+
 __global__ void k_fill_double(double *out, std::size_t n, double value)
 {
     const std::size_t i = static_cast<std::size_t>(blockIdx.x) * blockDim.x + threadIdx.x;

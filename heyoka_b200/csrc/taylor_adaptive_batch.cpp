@@ -114,6 +114,11 @@ struct taylor_adaptive_batch<double>::impl {
     std::vector<t_event_batch<double>> tes;
     std::vector<nt_event_batch<double>> ntes;
     std::vector<std::vector<std::optional<std::pair<double, double>>>> te_cooldowns; // filled by get_te_cooldowns()
+    // Variational integrators (var_ode_sys): order (0 = not variational), arguments, original state variables, and
+    // the last Taylor map [n_orig_sv][batch].
+    std::uint32_t vorder = 0, n_orig_sv = 0;
+    std::vector<expression> vargs;
+    std::vector<double> tstate;
     // Host <-> device synchronisation (see host_sync in taylor.hpp). strict: everything is uploaded at the entry of
     // every call and refreshed at its exit (the reference's raw-pointer contract). lazy: an array is uploaded only
     // after the user could have written it (non-const getters, setters), and the mirrors are refreshed when a getter
@@ -158,7 +163,8 @@ struct taylor_adaptive_batch<double>::impl {
           tape_mode(o.tape_mode), k_lpw(o.k_lpw), k_lpt(o.k_lpt), k_threads(o.k_threads), k_bpsm(o.k_bpsm),
           state(o.state), pars(o.pars), time_hi(o.time_hi), time_lo(o.time_lo), tc(o.tc), last_h(o.last_h),
           d_out(o.d_out), step_res(o.step_res), prop_res(o.prop_res), oc(o.oc), tmp_a(o.tmp_a), tmp_b(o.tmp_b),
-          tmp_n(o.tmp_n), tc_valid(o.tc_valid), tes(o.tes), ntes(o.ntes), lazy(o.lazy)
+          tmp_n(o.tmp_n), tc_valid(o.tc_valid), tes(o.tes), ntes(o.ntes), vorder(o.vorder), n_orig_sv(o.n_orig_sv),
+          vargs(o.vargs), tstate(o.tstate), lazy(o.lazy)
     {
         if (prog) {
             make_batch();
@@ -473,6 +479,35 @@ void taylor_adaptive_batch<double>::finalise_ctor(std::vector<std::pair<expressi
     }
 }
 
+void taylor_adaptive_batch<double>::finalise_ctor(const var_ode_sys &vsys, std::vector<double> state,
+                                                  std::uint32_t batch_size, ctor_opts o)
+{
+    const auto n_orig = static_cast<std::size_t>(vsys.get_n_orig_sv());
+    const auto &vargs = vsys.get_vargs();
+    const auto &aug = vsys.get_sys();
+    const auto n = static_cast<std::size_t>(batch_size);
+    if (batch_size != 0u && (state.empty() || state.size() == n_orig * n)) {
+        // The variational rows: per lane, column j of the STM is e_k when argument j is the state variable x_k, 0 when
+        // it is a parameter (dx(t0)/dx_k(t0) = e_k, dx(t0)/dp = 0).
+        state.resize(aug.size() * n, 0.);
+        for (std::size_t i = 0; i < n_orig; ++i) {
+            for (std::size_t j = 0; j < vargs.size(); ++j) {
+                if (vargs[j] == aug[i].first) {
+                    const auto row = n_orig + i * vargs.size() + j;
+                    std::fill(state.begin() + static_cast<std::ptrdiff_t>(row * n),
+                              state.begin() + static_cast<std::ptrdiff_t>((row + 1u) * n), 1.);
+                }
+            }
+        }
+    }
+    finalise_ctor(aug, std::move(state), batch_size, std::move(o));
+    auto &m = *m_impl;
+    m.vorder = vsys.get_order();
+    m.n_orig_sv = vsys.get_n_orig_sv();
+    m.vargs = vargs;
+    m.tstate.assign(n_orig * n, 0.);
+}
+
 const taylor_dc_t &taylor_adaptive_batch<double>::get_decomposition() const
 {
     return m_impl->dc;
@@ -503,15 +538,107 @@ std::uint32_t taylor_adaptive_batch<double>::get_dim() const
 }
 bool taylor_adaptive_batch<double>::is_variational() const noexcept
 {
-    return false;
+    return m_impl->vorder != 0u;
 }
 std::uint32_t taylor_adaptive_batch<double>::get_n_orig_sv() const noexcept
 {
-    return m_impl->dim;
+    return m_impl->vorder != 0u ? m_impl->n_orig_sv : m_impl->dim;
 }
 const std::vector<std::pair<expression, expression>> &taylor_adaptive_batch<double>::get_sys() const noexcept
 {
     return m_impl->sys;
+}
+std::uint32_t taylor_adaptive_batch<double>::get_vorder() const noexcept
+{
+    return m_impl->vorder;
+}
+const std::vector<expression> &taylor_adaptive_batch<double>::get_vargs() const noexcept
+{
+    return m_impl->vargs;
+}
+
+namespace
+{
+
+void check_variational(std::uint32_t vorder, const char *what)
+{
+    if (vorder == 0u) {
+        throw std::invalid_argument(std::string("The function ") + what
+                                    + " can be invoked only on a variational integrator");
+    }
+}
+
+} // namespace
+
+std::pair<std::uint32_t, std::uint32_t> taylor_adaptive_batch<double>::get_vslice(std::uint32_t order) const
+{
+    const auto &m = *m_impl;
+    check_variational(m.vorder, "get_vslice()");
+    if (order > m.vorder) {
+        throw std::invalid_argument("Cannot fetch the slice of the derivatives of order " + std::to_string(order)
+                                    + " in a variational integrator of order " + std::to_string(m.vorder));
+    }
+    return order == 0u ? std::pair{0u, m.n_orig_sv} : std::pair{m.n_orig_sv, m.dim};
+}
+
+std::pair<std::uint32_t, std::uint32_t> taylor_adaptive_batch<double>::get_vslice(std::uint32_t component,
+                                                                                  std::uint32_t order) const
+{
+    const auto &m = *m_impl;
+    const auto all = get_vslice(order);
+    if (component >= m.n_orig_sv) {
+        throw std::invalid_argument("Cannot fetch the slice of the derivatives of the component "
+                                    + std::to_string(component) + " in a variational integrator with "
+                                    + std::to_string(m.n_orig_sv) + " original state variables");
+    }
+    if (order == 0u) {
+        return {component, component + 1u};
+    }
+    const auto n_args = static_cast<std::uint32_t>(m.vargs.size());
+    return {all.first + component * n_args, all.first + (component + 1u) * n_args};
+}
+
+std::vector<std::uint32_t> taylor_adaptive_batch<double>::get_mindex(std::uint32_t i) const
+{
+    const auto &m = *m_impl;
+    check_variational(m.vorder, "get_mindex()");
+    if (i >= m.dim) {
+        throw std::invalid_argument("Cannot fetch the multi-index of the state variable " + std::to_string(i)
+                                    + " in a variational integrator with " + std::to_string(m.dim)
+                                    + " state variables");
+    }
+    const auto n_args = static_cast<std::uint32_t>(m.vargs.size());
+    std::vector<std::uint32_t> ret(1u + n_args, 0u);
+    if (i < m.n_orig_sv) {
+        ret[0] = i;
+    } else {
+        ret[0] = (i - m.n_orig_sv) / n_args;
+        ret[1u + (i - m.n_orig_sv) % n_args] = 1u;
+    }
+    return ret;
+}
+
+const std::vector<double> &taylor_adaptive_batch<double>::eval_taylor_map(const std::vector<double> &dx)
+{
+    auto &m = *m_impl;
+    check_variational(m.vorder, "eval_taylor_map()");
+    const auto n_args = static_cast<std::uint32_t>(m.vargs.size());
+    if (dx.size() != static_cast<std::size_t>(n_args) * m.batch_size) {
+        throw std::invalid_argument("Invalid number of values passed to eval_taylor_map(): "
+                                    + std::to_string(dx.size()) + " values were passed, but "
+                                    + std::to_string(static_cast<std::size_t>(n_args) * m.batch_size)
+                                    + " are needed (" + std::to_string(n_args) + " arguments in batches of "
+                                    + std::to_string(m.batch_size) + ")");
+    }
+    // The map is evaluated from the state the user sees (the host mirror in strict mode).
+    m.push();
+    check(hy_batch_eval_taylor_map(m.batch, m.n_orig_sv, n_args, dx.data(), m.tstate.data(), 0));
+    return m.tstate;
+}
+
+const std::vector<double> &taylor_adaptive_batch<double>::get_tstate() const noexcept
+{
+    return m_impl->tstate;
 }
 const std::vector<double> &taylor_adaptive_batch<double>::get_time() const
 {

@@ -70,6 +70,21 @@ hy_ex *hy_ex_copy(const hy_ex *);
 void hy_ex_free(hy_ex *);
 /* Writes a NUL-terminated rendering into buf (truncated to buf_len); returns the full length. */
 size_t hy_ex_str(const hy_ex *, char *buf, size_t buf_len);
+/* Symbolic derivative of e with respect to wrt (a variable or a parameter); NULL on error (hy_last_error()). */
+hy_ex *hy_ex_diff(const hy_ex *e, const hy_ex *wrt);
+
+/* Variational ODE system of order 1 (heyoka_b200/var_ode_sys.hpp: layout, names, right-hand sides). The arguments:
+ * flags != 0 selects them with HY_VAR_ARGS_* bits (args ignored); flags == 0 takes the n_args expressions of args,
+ * state variables and / or parameters, in the order given. The augmented system has *n_out_eq = n_eq * (1 + m)
+ * equations and *n_out_args = m arguments. out_lhs / out_rhs / out_args == NULL: only the two counts are written;
+ * otherwise they receive *n_out_eq, *n_out_eq and *n_out_args new handles (the caller frees each with hy_ex_free).
+ * Order > 1 and the time argument: HY_ERR_NOT_IMPLEMENTED. */
+#define HY_VAR_ARGS_VARS 1u
+#define HY_VAR_ARGS_PARAMS 2u
+#define HY_VAR_ARGS_TIME 4u
+int hy_var_ode_sys(const hy_ex *const *lhs, const hy_ex *const *rhs, uint32_t n_eq, uint32_t flags,
+                   const hy_ex *const *args, uint32_t n_args, uint32_t order, uint32_t *n_out_eq, uint32_t *n_out_args,
+                   hy_ex **out_lhs, hy_ex **out_rhs, hy_ex **out_args);
 
 /* Model builders (src/model/nbody.cpp:53-173, src/model/pendulum.cpp:24-29, src/model/ffnn.cpp:70-142).
  * They fill lhs[i]/rhs[i] (caller frees each with hy_ex_free). */
@@ -331,6 +346,15 @@ void hy_cout_destroy(hy_cout *);
 /* Dense output from the last written tc: out[var * batch + lane] = sum_o tc[var][o][lane] * tau[lane]^o
  * (src/taylor_01.cpp:1015-1185; tau relative to the start of the last step). out/tau are host arrays. */
 int hy_batch_d_output(hy_batch *, const double *tau, double *out);
+
+/* Taylor map of a variational batch of order 1 (hy_var_ode_sys()): with the current state x (rows 0..n_orig_sv) and
+ * state-transition matrix Phi (rows n_orig_sv.., component-major), out[i * batch + lane] = x_i + sum_j Phi_ij dx_j for
+ * dx[j * batch + lane], j < n_args. Requires n_orig_sv * (1 + n_args) == n_eq. The sum starts from x_i and adds the
+ * rounded products in the order j = 0 .. n_args - 1, each rounded, with no contraction. on_device != 0: dx and out are
+ * device pointers (not available on a multi-device batch), the kernel is enqueued on the batch's stream and the call
+ * returns without waiting (hy_batch_sync()); else host arrays, and the call returns with out written. */
+int hy_batch_eval_taylor_map(hy_batch *, uint32_t n_orig_sv, uint32_t n_args, const double *dx, double *out,
+                             int on_device);
 
 /* ------------------------------------------------------------------------------------------------
  * E. Event detection in batch mode.

@@ -214,6 +214,12 @@ std::vector<std::string> get_variables(const expression &);
 std::uint32_t get_param_size(const std::vector<expression> &);
 bool is_time_dependent(const std::vector<expression> &);
 
+// Symbolic derivative of e with respect to wrt, a variable or a parameter par[i] (heyoka's diff(), restated from
+// its documented rules: the reference's source is not in this tree). Every result is built through the folding
+// builders sum() / prod() / pow(), so that zeros and ones fold away. The functions that only the decomposition
+// creates (sub, div, sum_sq, num_identity) are refused with std::invalid_argument.
+expression diff(const expression &e, const expression &wrt);
+
 } // namespace heyoka_b200
 
 namespace std

@@ -9,5 +9,6 @@
 #include <heyoka_b200/model.hpp>
 #include <heyoka_b200/taylor.hpp>
 #include <heyoka_b200/taylor_decompose.hpp>
+#include <heyoka_b200/var_ode_sys.hpp>
 
 #endif
