@@ -1598,6 +1598,20 @@ static void ed_add_d_event(const double *ptr, uint32_t order, double h, int dir,
     }
 }
 
+/* Deepest working list of the root isolation since the last oracle_ev_max_depth_w1(1) call. A readout for the tests: the
+ * device keeps this list in a fixed stack of EV_STACK entries (ev_kernels.cuh), the reference in a list it gives up on
+ * past 250 entries. Not read by anything else. */
+static uint32_t ed_max_wl = 0u;
+
+uint32_t oracle_ev_max_depth_w1(int reset)
+{
+    const uint32_t ret = ed_max_wl;
+    if (reset) {
+        ed_max_wl = 0u;
+    }
+    return ret;
+}
+
 /* The body of run_detection() (:1767-2168) for one batch element and one event: the polynomial of the event is
  * ptr[0..order], dir the requested direction, cd = {time in cooldown, cooldown} or NULL. */
 static void ed_detect_one(const double *ptr, uint32_t order, double h, double g_eps, int dir, const double *cd,
@@ -1663,6 +1677,7 @@ static void ed_detect_one(const double *ptr, uint32_t order, double h, double g_
             wl_b[2u * n_wl + 1u] = ub;
             memcpy(wl_p + (size_t)n_wl * np1, tmp2, sizeof(double) * np1);
             ++n_wl;
+            ed_max_wl = n_wl > ed_max_wl ? n_wl : ed_max_wl;
         }
         if (n_wl > 250u || n_isol > order) {
             loop_failed = 1;

@@ -449,6 +449,13 @@ class OracleBatch:
         return out
 
 
+def ev_max_depth(reset=True):
+    """Deepest working list of the oracle's root isolation (entries held at once) since the last reset; the device
+    holds that list in a stack of dev::EV_STACK entries."""
+    lib.oracle_ev_max_depth_w1.restype = C.c_uint32
+    return int(lib.oracle_ev_max_depth_w1(C.c_int(1 if reset else 0)))
+
+
 _OEI = None
 
 
