@@ -232,9 +232,12 @@ struct candidate {
 } // namespace
 
 // ------------------------------------------------------------------------------------------------
-// Host object.
+// Host objects: a shard is the device state of one block of lanes on one device; a hy_batch is one or more shards.
 // ------------------------------------------------------------------------------------------------
-struct hy_batch {
+namespace
+{
+
+struct shard {
     int device = 0;
     cudaStream_t stream = nullptr;
     std::uint32_t n = 0;
@@ -274,13 +277,11 @@ struct hy_batch {
 
     // Event detection (section E of the C ABI; ev_kernels.cuh). n_ev > 0: the program carries event equations, every
     // step is an event step (jet without propagation + detection + propagation cut at the first terminal event).
-    std::uint32_t n_ev = 0, n_te = 0;
-    bool ev_set = false;
+    std::uint32_t n_ev = 0;
     dev::ev_args eva{};
     std::vector<void *> ev_allocs;
-    std::vector<hy_event_rec> ev_host; // the events of the last step, in the order the callbacks must run
-    void ev_setup(std::uint32_t n_te_, const std::int32_t *dirs, const double *cooldowns, double tol);
-    void ev_step(const double *max_delta_t, int on_device, int backward);
+    void ev_setup(std::uint32_t n_te, const std::int32_t *dirs, const double *cooldowns, double tol);
+    std::vector<hy_event_rec> ev_step(const double *max_delta_t, int backward);
 
     // Resident arrays.
     double *d_state = nullptr, *d_pars = nullptr, *d_t_hi = nullptr, *d_t_lo = nullptr, *d_last_h = nullptr,
@@ -307,12 +308,7 @@ struct hy_batch {
     std::uint32_t h_threads = 256; // CTA size of k_hbm when a request gives none: the last one given
     std::uint64_t n_launches = 0;
 
-    // Multi-device batch (hy_batch_create_multi()): the parent owns no device memory, only one single-device hy_batch
-    // per shard of contiguous lanes [shard_off[i], shard_off[i + 1]).
-    std::vector<hy_batch *> shards;
-    std::vector<std::uint32_t> shard_off;
-
-    ~hy_batch();
+    ~shard();
     void free_all() noexcept;
     dev::batch view() const;
     template <typename T>
@@ -331,8 +327,24 @@ struct hy_batch {
     void launch(bool prop, const dev::run_args &R);
 };
 
+} // namespace
+
+// Lanes [off[i], off[i + 1]) of the batch live on shards[i]; host arrays are batch-innermost ([row][batch]), so a
+// shard's slice of a row is contiguous and its copies are pitched 2D copies.
+struct hy_batch {
+    std::vector<std::unique_ptr<shard>> shards; // at least one
+    std::vector<std::uint32_t> off;
+    std::uint32_t n = 0, n_eq = 0;
+    bool multi = false; // created by hy_batch_create_multi(), whatever its number of shards
+    // Events: every shard detects the events of its own lanes; ev_host holds those of the last step for the whole
+    // batch, in the order the callbacks must run.
+    std::uint32_t n_ev = 0, n_te = 0;
+    bool ev_set = false;
+    std::vector<hy_event_rec> ev_host;
+};
+
 template <typename T>
-T *hy_batch::dalloc(std::size_t count)
+T *shard::dalloc(std::size_t count)
 {
     void *p = nullptr;
     HY_CUDA_CHECK(cudaMalloc(&p, std::max<std::size_t>(count, 1u) * sizeof(T)));
@@ -340,7 +352,7 @@ T *hy_batch::dalloc(std::size_t count)
 }
 
 template <typename T>
-T *hy_batch::dupload(const std::vector<T> &v)
+T *shard::dupload(const std::vector<T> &v)
 {
     T *p = dalloc<T>(v.size());
     if (!v.empty()) {
@@ -349,7 +361,7 @@ T *hy_batch::dupload(const std::vector<T> &v)
     return p;
 }
 
-void hy_batch::free_all() noexcept
+void shard::free_all() noexcept
 {
     for (void *p :
          {static_cast<void *>(d_ops), static_cast<void *>(d_args), static_cast<void *>(d_sv_defs),
@@ -376,14 +388,8 @@ void hy_batch::free_all() noexcept
     ev_allocs.clear();
 }
 
-hy_batch::~hy_batch()
+shard::~shard()
 {
-    for (auto *sh : shards) {
-        delete sh;
-    }
-    if (!shards.empty()) {
-        return;
-    }
     int cur = 0;
     if (cudaGetDevice(&cur) == cudaSuccess) {
         cudaSetDevice(device);
@@ -392,7 +398,7 @@ hy_batch::~hy_batch()
     }
 }
 
-dev::batch hy_batch::view() const
+dev::batch shard::view() const
 {
     dev::batch b{};
     b.n = n;
@@ -412,14 +418,14 @@ dev::batch hy_batch::view() const
 }
 
 // Device memory that is free once the current selection's scratch is released.
-std::size_t hy_batch::free_bytes_after_release() const
+std::size_t shard::free_bytes_after_release() const
 {
     std::size_t free_b = 0, total_b = 0;
     HY_CUDA_CHECK(cudaMemGetInfo(&free_b, &total_b));
     return free_b + (sel.gscratch + sel.cscratch) * sizeof(double);
 }
 
-void hy_batch::setup_hbm(std::uint32_t threads, std::uint32_t blocks_per_sm, candidate &c) const
+void shard::setup_hbm(std::uint32_t threads, std::uint32_t blocks_per_sm, candidate &c) const
 {
     if (threads == 0u) {
         threads = h_threads;
@@ -448,7 +454,7 @@ void hy_batch::setup_hbm(std::uint32_t threads, std::uint32_t blocks_per_sm, can
            static_cast<std::size_t>(grid) * warps_per_block * slab_doubles};
 }
 
-coop_tables hy_batch::make_tables(bool spill) const
+coop_tables shard::make_tables(bool spill) const
 {
     coop_tables t;
     t.plan = hy::detail::make_smem_plan(*prog_host, opt_fuse, opt_fuse_sv, spill);
@@ -457,7 +463,7 @@ coop_tables hy_batch::make_tables(bool spill) const
     return t;
 }
 
-void hy_batch::set_tables(coop_tables t)
+void shard::set_tables(coop_tables t)
 {
     if (d_blob != nullptr) {
         HY_CUDA_CHECK(cudaFree(d_blob));
@@ -470,7 +476,7 @@ void hy_batch::set_tables(coop_tables t)
 
 // Returns false if the requested / any configuration does not fit in shared memory.
 // L = lanes per warp, N = lanes per thread, threads = 32 x warps per block.
-bool hy_batch::setup_coop(int L, int N, std::uint32_t threads, std::uint32_t ctas_per_sm, candidate &c) const
+bool shard::setup_coop(int L, int N, std::uint32_t threads, std::uint32_t ctas_per_sm, candidate &c) const
 {
     const std::size_t reserve = 1024u; // per-block reservation of the driver
     if (N == 0) {
@@ -571,7 +577,7 @@ bool hy_batch::setup_coop(int L, int N, std::uint32_t threads, std::uint32_t cta
 // bodies: 56k doubles per lane): same program, same planner, but every warp's tape is a slab of global memory and
 // the tables are read in place. Unlike the one-thread-per-lane HBM-tape kernel it fills the GPU with a few
 // thousand lanes (a warp works on L lanes, its threads on different u variables).
-void hy_batch::setup_coop_global(int L, int N, std::uint32_t threads, int cta, candidate &c) const
+void shard::setup_coop_global(int L, int N, std::uint32_t threads, int cta, candidate &c) const
 {
     c.tables.reset();
     if (plan.n_gslots != 0u) {
@@ -688,7 +694,7 @@ static bool make_nb1_tab(const hy::detail::nb_plan &pl, std::uint32_t n_eq, std:
 // The dedicated N-body kernel. LT = lanes per team (0: as many as give every thread of a warp one pair interaction),
 // threads = CTA size (0: as many warps as fit; HEYOKA_B200_NB_THREADS caps it), want_cta: -1 automatic.
 // Returns false if the program does not qualify or nothing fits.
-bool hy_batch::setup_nb(int LT, std::uint32_t threads, int want_cta, int want_lane, candidate &c) const
+bool shard::setup_nb(int LT, std::uint32_t threads, int want_cta, int want_lane, candidate &c) const
 {
     if (!nbp.ok) {
         return false;
@@ -842,7 +848,7 @@ bool hy_batch::setup_nb(int LT, std::uint32_t threads, int want_cta, int want_la
 // The dense-network kernel: the padded shared-memory image of the weights is prepared here (row pitch = 4 mod 16
 // doubles: the 8 x 4 A fragments of the tensor-core products then read conflict-free), copied once per CTA by the TMA
 // unit. Returns false if the program is not a network or does not fit in shared memory.
-bool hy_batch::setup_nn(candidate &c) const
+bool shard::setup_nn(candidate &c) const
 {
     if (!nnp.ok || nnp.layers.size() > static_cast<std::size_t>(dev::NN_MAX_LAYERS)) {
         return false;
@@ -898,7 +904,7 @@ bool hy_batch::setup_nn(candidate &c) const
 
 // The kernel a request selects (tape_mode as hy_batch_set_kernel() takes it, 0 automatic). A request that cannot run
 // throws, and leaves the batch as it is.
-candidate hy_batch::decide(int want_mode, int L, int N, std::uint32_t threads, std::uint32_t blocks_per_sm) const
+candidate shard::decide(int want_mode, int L, int N, std::uint32_t threads, std::uint32_t blocks_per_sm) const
 {
     candidate c;
     // Mode 8: the dense-network kernel (right-hand sides that are feed-forward networks, nn_plan.hpp); the automatic
@@ -952,7 +958,7 @@ candidate hy_batch::decide(int want_mode, int L, int N, std::uint32_t threads, s
 
 // Installs a decided selection: releases the scratch of the current one, uploads the tables of the new one and
 // allocates its scratch. Only CUDA errors can fail here.
-void hy_batch::commit(candidate c)
+void shard::commit(candidate c)
 {
     const auto release = [](auto *&p) {
         if (p != nullptr) {
@@ -998,7 +1004,7 @@ void hy_batch::commit(candidate c)
 // The public Taylor-coefficient array, [n_eq][order + 1][batch] (src/taylor_00.cpp:574-580), is allocated the first
 // time something needs it (write_tc, dense output, hy_batch_get_ptrs()): 6-body, 2^20 lanes: 6.3 GB; the
 // cooperative kernels keep the coefficients of the current step in a private per-warp store otherwise.
-void hy_batch::ensure_tc()
+void shard::ensure_tc()
 {
     if (d_tc == nullptr) {
         // (With events, the rows of the event equations follow those of the state variables.)
@@ -1009,24 +1015,9 @@ void hy_batch::ensure_tc()
 }
 
 // ---- Event detection (ev_kernels.cuh) ----
-void hy_batch::ev_setup(std::uint32_t n_te_, const std::int32_t *dirs, const double *cooldowns, double tol)
+// (The arguments are checked by hy_batch_set_events().)
+void shard::ev_setup(std::uint32_t n_te, const std::int32_t *dirs, const double *cooldowns, double tol)
 {
-    if (n_ev == 0u) {
-        throw std::invalid_argument("This batch was built from a program without event equations");
-    }
-    if (n_te_ > n_ev) {
-        throw std::invalid_argument("The number of terminal events exceeds the number of event equations");
-    }
-    for (std::uint32_t k = 0; k < n_ev; ++k) {
-        if (dirs[k] < -1 || dirs[k] > 1) {
-            throw std::invalid_argument("Invalid value selected for the direction of an event");
-        }
-    }
-    for (std::uint32_t k = 0; k < n_te_; ++k) {
-        if (!std::isfinite(cooldowns[k])) {
-            throw std::invalid_argument("Cannot set a non-finite cooldown value for a terminal event");
-        }
-    }
     for (void *q : ev_allocs) {
         HY_CUDA_CHECK(cudaFree(q));
     }
@@ -1035,7 +1026,6 @@ void hy_batch::ev_setup(std::uint32_t n_te_, const std::int32_t *dirs, const dou
         ev_allocs.push_back(static_cast<void *>(q));
         return q;
     };
-    n_te = n_te_;
     const std::uint32_t p = order, pp1 = p + 1u;
     dev::ev_args E{};
     E.n_ev = n_ev;
@@ -1073,15 +1063,11 @@ void hy_batch::ev_setup(std::uint32_t n_te_, const std::int32_t *dirs, const dou
     E.arena_threads = 64u * std::min<std::uint32_t>(n_sms, static_cast<std::uint32_t>((B * n_ev + 63u) / 64u));
     E.arena = keep(dalloc<double>(static_cast<std::size_t>(dev::EV_STACK) * (pp1 + 2u) * E.arena_threads));
     eva = E;
-    ev_set = true;
-    ev_host.clear();
 }
 
-void hy_batch::ev_step(const double *d_mdt, int, int backward)
+// One event step; returns the events found, in the order the callbacks must run.
+std::vector<hy_event_rec> shard::ev_step(const double *d_mdt, int backward)
 {
-    if (!ev_set) {
-        throw std::invalid_argument("hy_batch_set_events() must be called before stepping a batch with event equations");
-    }
     if (sel.family != kernel_sel::hbm) {
         commit(decide(1, 0, 0, 0, 0));
     }
@@ -1130,7 +1116,7 @@ void hy_batch::ev_step(const double *d_mdt, int, int backward)
     }
     dev::k_ev_apply<<<(B + 127u) / 128u, 128, 0, stream>>>(prog, view(), eva);
     ++n_launches;
-    ev_host.clear();
+    std::vector<hy_event_rec> evs;
     if (n_rec != 0u) {
         dev::k_ev_filter<<<(n_rec + 127u) / 128u, 128, 0, stream>>>(view(), eva);
         ++n_launches;
@@ -1139,12 +1125,12 @@ void hy_batch::ev_step(const double *d_mdt, int, int backward)
         HY_CUDA_CHECK(cudaStreamSynchronize(stream));
         for (const auto &r : recs) {
             if (r.live != 0u) {
-                ev_host.push_back(hy_event_rec{r.lane, r.idx, r.terminal, r.d_sgn, r.t, r.abs_der});
+                evs.push_back(hy_event_rec{r.lane, r.idx, r.terminal, r.d_sgn, r.t, r.abs_der});
             }
         }
         // Per lane: the non-terminal events in time order (src/taylor_adaptive_batch.cpp:789-790: by |t|; equal times
         // keep the order of the event indices), then the terminal event.
-        std::sort(ev_host.begin(), ev_host.end(), [](const hy_event_rec &a, const hy_event_rec &b) {
+        std::sort(evs.begin(), evs.end(), [](const hy_event_rec &a, const hy_event_rec &b) {
             if (a.lane != b.lane) {
                 return a.lane < b.lane;
             }
@@ -1158,9 +1144,10 @@ void hy_batch::ev_step(const double *d_mdt, int, int backward)
         });
     }
     HY_CUDA_CHECK(cudaGetLastError());
+    return evs;
 }
 
-void hy_batch::launch(bool prop, const dev::run_args &R)
+void shard::launch(bool prop, const dev::run_args &R)
 {
     if (R.write_tc != 0) {
         ensure_tc();
@@ -1219,148 +1206,184 @@ struct device_guard {
     }
 };
 
-// Stage a host (or device) array of n doubles into slot `slot` of d_tmp; returns the device pointer.
-const double *stage(hy_batch *b, const double *src, int on_device, std::uint32_t slot)
+// The device state of `lanes` lanes of the program on `device`.
+std::unique_ptr<shard> make_shard(const hy_program &p, std::uint32_t lanes, int device)
 {
-    if (src == nullptr) {
-        return nullptr;
+    // Overflow checks on the buffer sizes, like src/taylor_adaptive_batch.cpp:256-264,375-378.
+    const std::uint64_t tc_size = static_cast<std::uint64_t>(p.n_eq) * (p.order + 1u) * lanes;
+    if (tc_size > (std::numeric_limits<std::uint64_t>::max() >> 4)) {
+        throw std::overflow_error("Overflow detected while computing the size of the Taylor coefficients buffer");
     }
-    if (on_device) {
-        return src;
+
+    auto sh = std::make_unique<shard>();
+    sh->device = device;
+    device_guard guard(device);
+
+    sh->n = lanes;
+    sh->n_eq = p.n_eq;
+    sh->n_pars = p.n_pars;
+    sh->order = p.order;
+    sh->n_uvars = p.n_uvars;
+    sh->high_accuracy = p.high_accuracy;
+
+    cudaDeviceProp prop{};
+    HY_CUDA_CHECK(cudaGetDeviceProperties(&prop, device));
+    sh->n_sms = static_cast<std::uint32_t>(prop.multiProcessorCount);
+    sh->smem_per_block_max = prop.sharedMemPerBlockOptin;
+    sh->smem_per_sm = prop.sharedMemPerMultiprocessor;
+
+    // Program arrays, "hbm" encoding.
+    static_assert(sizeof(hy_op) == sizeof(uint4), "hy_op must be 16 bytes");
+    sh->d_ops = reinterpret_cast<uint4 *>(sh->dupload(p.ops));
+    sh->d_args = sh->dupload(p.args);
+    sh->d_consts = sh->dupload(p.consts);
+    sh->d_sv_defs = sh->dupload(p.sv_defs);
+
+    auto &P = sh->prog;
+    P.n_eq = p.n_eq;
+    P.n_uvars = p.n_uvars;
+    P.n_pars = p.n_pars;
+    P.order = p.order;
+    P.n_ops = p.n_uvars - p.n_eq;
+    P.high_accuracy = p.high_accuracy ? 1 : 0;
+    // taylor_determine_h_rhofac(), src/taylor_00.cpp:84-94 (host libm, like the reference's number arithmetic).
+    P.rhofac = std::exp((-7. / 10.) / static_cast<double>(p.order - 1u)) / (std::exp(1.) * std::exp(1.));
+    P.inv_p = 1. / static_cast<double>(p.order);
+    P.inv_pm1 = 1. / static_cast<double>(p.order - 1u);
+    P.ops = sh->d_ops;
+    P.args = sh->d_args;
+    P.consts = sh->d_consts;
+    P.sv_defs = sh->d_sv_defs;
+
+    // Cooperative plan.
+    // HEYOKA_B200_FUSE=0 disables the superinstructions, HEYOKA_B200_FUSE_SV=0 the fused state-variable
+    // propagation, HEYOKA_B200_SPILL=0/1 forces the overflow tape off/on (diagnostics / tests).
+    if (const char *env = std::getenv("HEYOKA_B200_FUSE")) {
+        sh->opt_fuse = std::string{env} != "0";
     }
-    double *dst = b->d_tmp + static_cast<std::size_t>(slot) * b->n;
-    HY_CUDA_CHECK(cudaMemcpyAsync(dst, src, sizeof(double) * b->n, cudaMemcpyHostToDevice, b->stream));
-    return dst;
-}
-
-// propagate_until() on one device, in three phases so that a multi-device run (hy_multi_*) can apply the reference's
-// GLOBAL exits across its shards:
-//   phase 1  snapshot of (state, time), one launch of the propagate kernel, flags read back (synchronises);
-//   replay   if a lane of ANY shard went non-finite: restore the snapshot and re-run with the iteration count capped at
-//            the first such iteration (the reference stops EVERY lane there, src/taylor_adaptive_batch.cpp:1462-1467;
-//            lanes are independent, so the capped re-run reproduces it exactly);
-//   finish   iteration limit -> every lane reports step_limit (:1516-1526); the lanes that were done before the loop's
-//            last iteration K took zero-length steps in the reference: last_h = 0 and, with write_tc, Taylor
-//            coefficients re-expanded about the final state (one masked zero-length step).
-struct prop_ctx {
-    dev::run_args R{};
-    dev::run_flags fl{};
-};
-
-void propagate_phase1(hy_batch *b, const double *d_tf_hi, const double *d_tf_lo, const double *d_mdt, uint64_t max_steps,
-                      int write_tc, prop_ctx &c)
-{
-    const std::size_t state_doubles = static_cast<std::size_t>(b->n_eq) * b->n;
-    HY_CUDA_CHECK(cudaMemcpyAsync(b->d_snapshot, b->d_state, sizeof(double) * state_doubles, cudaMemcpyDeviceToDevice,
-                                  b->stream));
-    HY_CUDA_CHECK(cudaMemcpyAsync(b->d_snapshot + state_doubles, b->d_t_hi, sizeof(double) * b->n,
-                                  cudaMemcpyDeviceToDevice, b->stream));
-    HY_CUDA_CHECK(cudaMemcpyAsync(b->d_snapshot + state_doubles + b->n, b->d_t_lo, sizeof(double) * b->n,
-                                  cudaMemcpyDeviceToDevice, b->stream));
-    const dev::run_flags init{0u, 0u, ~0ull, 0ull};
-    HY_CUDA_CHECK(cudaMemcpyAsync(b->d_flags, &init, sizeof(init), cudaMemcpyHostToDevice, b->stream));
-    c.R = dev::run_args{};
-    c.R.max_delta_t = d_mdt;
-    c.R.tf_hi = d_tf_hi;
-    c.R.tf_lo = d_tf_lo;
-    c.R.iter_cap = max_steps;
-    c.R.replay = 0;
-    c.R.write_tc = write_tc;
-    c.R.flags = b->d_flags;
-    c.R.counter = b->d_counter;
-    b->launch(true, c.R);
-    HY_CUDA_CHECK(cudaMemcpyAsync(&c.fl, b->d_flags, sizeof(c.fl), cudaMemcpyDeviceToHost, b->stream));
-    HY_CUDA_CHECK(cudaStreamSynchronize(b->stream));
-}
-
-void propagate_replay(hy_batch *b, prop_ctx &c, unsigned long long cap)
-{
-    const std::size_t state_doubles = static_cast<std::size_t>(b->n_eq) * b->n;
-    HY_CUDA_CHECK(cudaMemcpyAsync(b->d_state, b->d_snapshot, sizeof(double) * state_doubles, cudaMemcpyDeviceToDevice,
-                                  b->stream));
-    HY_CUDA_CHECK(cudaMemcpyAsync(b->d_t_hi, b->d_snapshot + state_doubles, sizeof(double) * b->n,
-                                  cudaMemcpyDeviceToDevice, b->stream));
-    HY_CUDA_CHECK(cudaMemcpyAsync(b->d_t_lo, b->d_snapshot + state_doubles + b->n, sizeof(double) * b->n,
-                                  cudaMemcpyDeviceToDevice, b->stream));
-    const dev::run_flags init{0u, 0u, ~0ull, 0ull};
-    HY_CUDA_CHECK(cudaMemcpyAsync(b->d_flags, &init, sizeof(init), cudaMemcpyHostToDevice, b->stream));
-    c.R.iter_cap = cap;
-    c.R.replay = 1;
-    b->launch(true, c.R);
-    HY_CUDA_CHECK(cudaMemcpyAsync(&c.fl, b->d_flags, sizeof(c.fl), cudaMemcpyDeviceToHost, b->stream));
-    HY_CUDA_CHECK(cudaStreamSynchronize(b->stream));
-}
-
-void propagate_finish(hy_batch *b, bool any_nf, bool any_limit, unsigned long long loop_len, int write_tc)
-{
-    const std::uint32_t gb = (b->n + 255u) / 256u;
-    if (!any_nf && any_limit) {
-        dev::k_fill_outcome<<<gb, 256, 0, b->stream>>>(b->d_prop_outcome, b->n, HY_OUTCOME_STEP_LIMIT);
-        HY_CUDA_CHECK(cudaGetLastError());
-        ++b->n_launches;
+    if (const char *env = std::getenv("HEYOKA_B200_FUSE_SV")) {
+        sh->opt_fuse_sv = std::string{env} != "0";
     }
-    // Lanes that were done before the last iteration of the reference's loop.
-    unsigned *d_any = reinterpret_cast<unsigned *>(b->d_flags) + sizeof(dev::run_flags) / sizeof(unsigned);
-    HY_CUDA_CHECK(cudaMemsetAsync(d_any, 0, sizeof(unsigned), b->stream));
-    dev::k_prop_early<<<gb, 256, 0, b->stream>>>(b->d_prop_iters, loop_len, b->n, b->d_last_h, b->d_skip, b->d_tmp, d_any);
-    HY_CUDA_CHECK(cudaGetLastError());
-    ++b->n_launches;
-    if (write_tc != 0) {
-        unsigned any = 0;
-        HY_CUDA_CHECK(cudaMemcpyAsync(&any, d_any, sizeof(any), cudaMemcpyDeviceToHost, b->stream));
-        HY_CUDA_CHECK(cudaStreamSynchronize(b->stream));
-        if (any != 0u) {
-            dev::run_args R{};
-            R.max_delta_t = b->d_tmp; // zeros
-            R.write_tc = 1;
-            R.flags = b->d_flags;
-            R.counter = b->d_counter;
-            R.skip = b->d_skip;
-            b->launch(false, R);
+    if (const char *env = std::getenv("HEYOKA_B200_SPILL")) {
+        sh->opt_spill = std::string{env} != "0" ? 1 : 0;
+    }
+    if (const char *env = std::getenv("HEYOKA_B200_NB")) {
+        sh->opt_nb = std::string{env} != "0" ? 1 : 0;
+    }
+    if (const char *env = std::getenv("HEYOKA_B200_NB_LANE")) {
+        sh->opt_nb1 = std::string{env} != "0" ? 1 : 0;
+    }
+    if (const char *env = std::getenv("HEYOKA_B200_NB_THREADS")) {
+        sh->opt_nb_threads = static_cast<std::uint32_t>(std::atoi(env));
+    }
+    sh->prog_host = std::make_shared<const hy_program>(p);
+    sh->set_tables(sh->make_tables(false));
+    sh->slab_doubles = static_cast<std::size_t>(p.n_uvars) * (p.order + 1u) * 32u;
+    sh->nbp = hy::detail::make_nb_plan(p);
+    if (const char *env = std::getenv("HEYOKA_B200_NN")) {
+        sh->opt_nn = std::string{env} != "0" ? 1 : 0;
+    }
+    sh->nnp = hy::detail::make_nn_plan(p);
+
+    // Resident arrays.
+    const std::size_t n = lanes;
+    sh->d_state = sh->dalloc<double>(n * p.n_eq);
+    sh->d_pars = sh->dalloc<double>(n * p.n_pars);
+    sh->d_t_hi = sh->dalloc<double>(n);
+    sh->d_t_lo = sh->dalloc<double>(n);
+    sh->d_last_h = sh->dalloc<double>(n);
+    sh->d_d_out = sh->dalloc<double>(n * p.n_eq);
+    sh->d_step_outcome = sh->dalloc<long long>(n);
+    sh->d_prop_outcome = sh->dalloc<long long>(n);
+    sh->d_prop_min_h = sh->dalloc<double>(n);
+    sh->d_prop_max_h = sh->dalloc<double>(n);
+    sh->d_prop_n_steps = sh->dalloc<unsigned long long>(n);
+    sh->d_prop_iters = sh->dalloc<unsigned long long>(n);
+    sh->d_skip = sh->dalloc<unsigned char>(n);
+    sh->d_tmp = sh->dalloc<double>(3u * n);
+    sh->d_snapshot = sh->dalloc<double>(n * (p.n_eq + 2u));
+    sh->d_counter = sh->dalloc<unsigned int>(1);
+    sh->d_flags = sh->dalloc<dev::run_flags>(2); // (+ scratch words behind the flags)
+
+    HY_CUDA_CHECK(cudaMemset(sh->d_state, 0, sizeof(double) * n * p.n_eq));
+    HY_CUDA_CHECK(cudaMemset(sh->d_pars, 0, sizeof(double) * std::max<std::size_t>(n * p.n_pars, 1u)));
+    HY_CUDA_CHECK(cudaMemset(sh->d_t_hi, 0, sizeof(double) * n));
+    HY_CUDA_CHECK(cudaMemset(sh->d_t_lo, 0, sizeof(double) * n));
+    HY_CUDA_CHECK(cudaMemset(sh->d_last_h, 0, sizeof(double) * n));
+
+    // Kernel selection: HEYOKA_B200_TAPE = hbm | smem overrides the automatic choice.
+    int want = 0;
+    if (const char *env = std::getenv("HEYOKA_B200_TAPE")) {
+        const std::string s{env};
+        want = s == "hbm" ? 1 : (s == "smem" ? 2 : 0);
+    }
+    sh->n_ev = static_cast<std::uint32_t>(p.ev_defs.size());
+    if (sh->n_ev != 0u) {
+        // Event detection runs on the thread-per-lane kernel family (ev_kernels.cuh).
+        if (p.order + 1u > static_cast<std::uint32_t>(dev::EV_MAXP1)) {
+            throw hy::detail::not_implemented_error("Event detection supports Taylor orders up to "
+                                                    + std::to_string(dev::EV_MAXP1 - 1));
         }
+        want = 1;
     }
+    sh->commit(sh->decide(want, 0, 0, 0, 0));
+    return sh;
 }
 
-int propagate_impl(hy_batch *b, const double *d_tf_hi, const double *d_tf_lo, const double *d_mdt, uint64_t max_steps,
-                   int write_tc, int *any_flag)
+// A batch of `batch` lanes in contiguous blocks, as even as possible, one per entry of devs (< 0: the current device);
+// never more shards than lanes.
+std::unique_ptr<hy_batch> make_batch(const hy_program &p, std::uint32_t batch, const std::vector<int> &devs, int n_dev,
+                                     bool multi)
 {
-    prop_ctx c;
-    propagate_phase1(b, d_tf_hi, d_tf_lo, d_mdt, max_steps, write_tc, c);
-    if (c.fl.any_nf != 0u) {
-        propagate_replay(b, c, c.fl.min_nf_iter);
+    auto b = std::make_unique<hy_batch>();
+    b->n = batch;
+    b->n_eq = p.n_eq;
+    b->n_ev = static_cast<std::uint32_t>(p.ev_defs.size());
+    b->multi = multi;
+    const std::uint32_t ns = std::min<std::uint32_t>(static_cast<std::uint32_t>(devs.size()), batch);
+    b->off.push_back(0u);
+    for (std::uint32_t i = 0; i < ns; ++i) {
+        int device = devs[i];
+        if (device < 0) {
+            HY_CUDA_CHECK(cudaGetDevice(&device));
+        }
+        if (device >= n_dev) {
+            throw std::invalid_argument("Invalid CUDA device index " + std::to_string(device));
+        }
+        const std::uint32_t lanes = batch / ns + (i < batch % ns ? 1u : 0u);
+        b->shards.push_back(make_shard(p, lanes, device));
+        b->off.push_back(b->off.back() + lanes);
     }
-    propagate_finish(b, c.fl.any_nf != 0u, c.fl.any_limit != 0u, c.fl.max_iter, write_tc);
-    if (any_flag != nullptr) {
-        *any_flag = (c.fl.any_nf != 0u ? 1 : 0) | (c.fl.any_limit != 0u ? 2 : 0);
-    }
-    return HY_OK;
+    return b;
 }
 
-} // namespace
-
 // ------------------------------------------------------------------------------------------------
-// Multi-device batches: the lanes are independent ODE systems, so a batch shards over the GPUs of a box with no
-// data-path communication (src/ensemble_propagate.cpp:192-311 partitions its members over TBB threads the same way).
-// Every shard is a single-device hy_batch driven by its own host thread; host arrays are batch-innermost
-// ([row][batch]), so a shard's slice of a row is contiguous and the copies are pitched 2D copies. The only coupling is
-// the reference's GLOBAL exits of propagate_until() (non-finite state anywhere, iteration limit, length of the
-// lock-step loop), applied across the shards between the phases of propagate (see propagate_phase1()).
+// Every entry point runs on the shards of its batch: the lanes are independent ODE systems, so a batch shards over the
+// GPUs of a box with no data-path communication (src/ensemble_propagate.cpp:192-311 partitions its members over TBB
+// threads the same way). The only coupling is the reference's GLOBAL exits of propagate_until() (non-finite state
+// anywhere, iteration limit, length of the lock-step loop), applied across the shards between the phases of
+// propagate().
 // ------------------------------------------------------------------------------------------------
-namespace
-{
 
+// fn(shard, i) on every shard, under the shard's device. One shard: on the calling thread. More: one host thread per
+// shard, so that the shards' copies and kernels overlap. The first failure in shard order is rethrown as it was thrown.
 template <typename F>
 void for_each_shard(hy_batch *b, F &&fn)
 {
     const std::size_t ns = b->shards.size();
+    if (ns == 1u) {
+        device_guard guard(b->shards[0]->device);
+        fn(*b->shards[0], std::size_t(0));
+        return;
+    }
     std::vector<std::exception_ptr> errs(ns);
     std::vector<std::thread> thr;
     thr.reserve(ns);
     for (std::size_t i = 0; i < ns; ++i) {
         thr.emplace_back([&, i] {
             try {
-                hy_batch *sh = b->shards[i];
-                device_guard guard(sh->device);
+                shard &sh = *b->shards[i];
+                device_guard guard(sh.device);
                 fn(sh, i);
             } catch (...) {
                 errs[i] = std::current_exception();
@@ -1377,56 +1400,262 @@ void for_each_shard(hy_batch *b, F &&fn)
     }
 }
 
-// rows x (shard lanes) block of a host array with `pitch` elements per row, starting at column `off`.
+// rows x (shard lanes) block of a host array with `pitch` elements per row, starting at column `off`. (The shard of an
+// unsharded batch takes the same pitched copy, with pitch = width: no slower than a flat copy on an H100.)
 template <typename T>
-void rows_h2d(hy_batch *sh, T *dst, const T *src, std::size_t rows, std::size_t pitch, std::size_t off)
+void rows_h2d(shard &sh, T *dst, const T *src, std::size_t rows, std::size_t pitch, std::size_t off)
 {
     if (src != nullptr && rows != 0u) {
-        HY_CUDA_CHECK(cudaMemcpy2DAsync(dst, sizeof(T) * sh->n, src + off, sizeof(T) * pitch, sizeof(T) * sh->n, rows,
-                                        cudaMemcpyHostToDevice, sh->stream));
+        HY_CUDA_CHECK(cudaMemcpy2DAsync(dst, sizeof(T) * sh.n, src + off, sizeof(T) * pitch, sizeof(T) * sh.n, rows,
+                                        cudaMemcpyHostToDevice, sh.stream));
     }
 }
 template <typename T>
-void rows_d2h(hy_batch *sh, T *dst, const T *src, std::size_t rows, std::size_t pitch, std::size_t off)
+void rows_d2h(shard &sh, T *dst, const T *src, std::size_t rows, std::size_t pitch, std::size_t off)
 {
     if (dst != nullptr && rows != 0u) {
-        HY_CUDA_CHECK(cudaMemcpy2DAsync(dst + off, sizeof(T) * pitch, src, sizeof(T) * sh->n, sizeof(T) * sh->n, rows,
-                                        cudaMemcpyDeviceToHost, sh->stream));
+        HY_CUDA_CHECK(cudaMemcpy2DAsync(dst + off, sizeof(T) * pitch, src, sizeof(T) * sh.n, sizeof(T) * sh.n, rows,
+                                        cudaMemcpyDeviceToHost, sh.stream));
     }
 }
 
-int multi_propagate(hy_batch *b, const double *tf_hi, const double *tf_lo, const double *mdt, uint64_t max_steps,
-                    int write_tc)
+// The shard's lanes [off, off + n) of a per-lane array: a host array is staged into slot `slot` of d_tmp, a device
+// array (on_device, an unsharded batch's) is used in place.
+const double *stage(shard &sh, const double *src, int on_device, std::size_t off, std::uint32_t slot)
 {
-    const std::size_t ns = b->shards.size();
-    std::vector<prop_ctx> ctx(ns);
-    for_each_shard(b, [&](hy_batch *sh, std::size_t i) {
-        const std::size_t off = b->shard_off[i];
-        const double *d_hi = stage(sh, tf_hi + off, 0, 0);
-        const double *d_lo = stage(sh, tf_lo != nullptr ? tf_lo + off : nullptr, 0, 1);
-        const double *d_mdt = stage(sh, mdt != nullptr ? mdt + off : nullptr, 0, 2);
-        propagate_phase1(sh, d_hi, d_lo, d_mdt, max_steps, write_tc, ctx[i]);
+    if (src == nullptr || on_device) {
+        return src;
+    }
+    double *dst = sh.d_tmp + static_cast<std::size_t>(slot) * sh.n;
+    HY_CUDA_CHECK(cudaMemcpyAsync(dst, src + off, sizeof(double) * sh.n, cudaMemcpyHostToDevice, sh.stream));
+    return dst;
+}
+
+void download(hy_batch *b, double *state, double *t_hi, double *t_lo, double *last_h)
+{
+    for_each_shard(b, [&](shard &sh, std::size_t i) {
+        rows_d2h(sh, state, sh.d_state, sh.n_eq, b->n, b->off[i]);
+        rows_d2h(sh, t_hi, sh.d_t_hi, 1u, b->n, b->off[i]);
+        rows_d2h(sh, t_lo, sh.d_t_lo, 1u, b->n, b->off[i]);
+        rows_d2h(sh, last_h, sh.d_last_h, 1u, b->n, b->off[i]);
+        HY_CUDA_CHECK(cudaStreamSynchronize(sh.stream));
     });
-    bool any_nf = false;
-    unsigned long long cap = ~0ull;
-    for (const auto &c : ctx) {
-        if (c.fl.any_nf != 0u) {
-            any_nf = true;
-            cap = std::min(cap, c.fl.min_nf_iter);
+}
+
+// propagate_until() on one shard, in three phases so that the reference's GLOBAL exits apply across the shards:
+//   phase 1  snapshot of (state, time), one launch of the propagate kernel, flags read back (synchronises);
+//   replay   if a lane of ANY shard went non-finite: restore the snapshot and re-run with the iteration count capped at
+//            the first such iteration (the reference stops EVERY lane there, src/taylor_adaptive_batch.cpp:1462-1467;
+//            lanes are independent, so the capped re-run reproduces it exactly);
+//   finish   iteration limit -> every lane reports step_limit (:1516-1526); the lanes that were done before the loop's
+//            last iteration K took zero-length steps in the reference: last_h = 0 and, with write_tc, Taylor
+//            coefficients re-expanded about the final state (one masked zero-length step).
+struct prop_ctx {
+    dev::run_args R{};
+    dev::run_flags fl{};
+};
+
+void propagate_phase1(shard &sh, const double *d_tf_hi, const double *d_tf_lo, const double *d_mdt, uint64_t max_steps,
+                      int write_tc, prop_ctx &c)
+{
+    const std::size_t state_doubles = static_cast<std::size_t>(sh.n_eq) * sh.n;
+    HY_CUDA_CHECK(cudaMemcpyAsync(sh.d_snapshot, sh.d_state, sizeof(double) * state_doubles, cudaMemcpyDeviceToDevice,
+                                  sh.stream));
+    HY_CUDA_CHECK(cudaMemcpyAsync(sh.d_snapshot + state_doubles, sh.d_t_hi, sizeof(double) * sh.n,
+                                  cudaMemcpyDeviceToDevice, sh.stream));
+    HY_CUDA_CHECK(cudaMemcpyAsync(sh.d_snapshot + state_doubles + sh.n, sh.d_t_lo, sizeof(double) * sh.n,
+                                  cudaMemcpyDeviceToDevice, sh.stream));
+    const dev::run_flags init{0u, 0u, ~0ull, 0ull};
+    HY_CUDA_CHECK(cudaMemcpyAsync(sh.d_flags, &init, sizeof(init), cudaMemcpyHostToDevice, sh.stream));
+    c.R = dev::run_args{};
+    c.R.max_delta_t = d_mdt;
+    c.R.tf_hi = d_tf_hi;
+    c.R.tf_lo = d_tf_lo;
+    c.R.iter_cap = max_steps;
+    c.R.replay = 0;
+    c.R.write_tc = write_tc;
+    c.R.flags = sh.d_flags;
+    c.R.counter = sh.d_counter;
+    sh.launch(true, c.R);
+    HY_CUDA_CHECK(cudaMemcpyAsync(&c.fl, sh.d_flags, sizeof(c.fl), cudaMemcpyDeviceToHost, sh.stream));
+    HY_CUDA_CHECK(cudaStreamSynchronize(sh.stream));
+}
+
+void propagate_replay(shard &sh, prop_ctx &c, unsigned long long cap)
+{
+    const std::size_t state_doubles = static_cast<std::size_t>(sh.n_eq) * sh.n;
+    HY_CUDA_CHECK(cudaMemcpyAsync(sh.d_state, sh.d_snapshot, sizeof(double) * state_doubles, cudaMemcpyDeviceToDevice,
+                                  sh.stream));
+    HY_CUDA_CHECK(cudaMemcpyAsync(sh.d_t_hi, sh.d_snapshot + state_doubles, sizeof(double) * sh.n,
+                                  cudaMemcpyDeviceToDevice, sh.stream));
+    HY_CUDA_CHECK(cudaMemcpyAsync(sh.d_t_lo, sh.d_snapshot + state_doubles + sh.n, sizeof(double) * sh.n,
+                                  cudaMemcpyDeviceToDevice, sh.stream));
+    const dev::run_flags init{0u, 0u, ~0ull, 0ull};
+    HY_CUDA_CHECK(cudaMemcpyAsync(sh.d_flags, &init, sizeof(init), cudaMemcpyHostToDevice, sh.stream));
+    c.R.iter_cap = cap;
+    c.R.replay = 1;
+    sh.launch(true, c.R);
+    HY_CUDA_CHECK(cudaMemcpyAsync(&c.fl, sh.d_flags, sizeof(c.fl), cudaMemcpyDeviceToHost, sh.stream));
+    HY_CUDA_CHECK(cudaStreamSynchronize(sh.stream));
+}
+
+// ex: the flags of the whole batch (any_nf from phase 1, any_limit and max_iter from the last launch).
+void propagate_finish(shard &sh, const dev::run_flags &ex, int write_tc)
+{
+    const std::uint32_t gb = (sh.n + 255u) / 256u;
+    if (ex.any_nf == 0u && ex.any_limit != 0u) {
+        dev::k_fill_outcome<<<gb, 256, 0, sh.stream>>>(sh.d_prop_outcome, sh.n, HY_OUTCOME_STEP_LIMIT);
+        HY_CUDA_CHECK(cudaGetLastError());
+        ++sh.n_launches;
+    }
+    // Lanes that were done before the last iteration of the reference's loop.
+    unsigned *d_any = reinterpret_cast<unsigned *>(sh.d_flags) + sizeof(dev::run_flags) / sizeof(unsigned);
+    HY_CUDA_CHECK(cudaMemsetAsync(d_any, 0, sizeof(unsigned), sh.stream));
+    dev::k_prop_early<<<gb, 256, 0, sh.stream>>>(sh.d_prop_iters, ex.max_iter, sh.n, sh.d_last_h, sh.d_skip, sh.d_tmp,
+                                                 d_any);
+    HY_CUDA_CHECK(cudaGetLastError());
+    ++sh.n_launches;
+    if (write_tc != 0) {
+        unsigned any = 0;
+        HY_CUDA_CHECK(cudaMemcpyAsync(&any, d_any, sizeof(any), cudaMemcpyDeviceToHost, sh.stream));
+        HY_CUDA_CHECK(cudaStreamSynchronize(sh.stream));
+        if (any != 0u) {
+            dev::run_args R{};
+            R.max_delta_t = sh.d_tmp; // zeros
+            R.write_tc = 1;
+            R.flags = sh.d_flags;
+            R.counter = sh.d_counter;
+            R.skip = sh.d_skip;
+            sh.launch(false, R);
         }
     }
-    if (any_nf) {
-        // Every lane of every shard stops at the first iteration in which any lane went non-finite.
-        for_each_shard(b, [&](hy_batch *sh, std::size_t i) { propagate_replay(sh, ctx[i], cap); });
-    }
-    bool any_limit = false;
-    unsigned long long loop_len = 0;
+}
+
+// The host arrays of hy_batch_propagate_until_host() (NULL: not wanted).
+struct prop_host {
+    const double *state_in, *pars, *t_hi_in, *t_lo_in;
+    double *state, *t_hi, *t_lo, *last_h;
+    int64_t *outcome;
+    double *min_h, *max_h;
+    uint64_t *n_steps;
+};
+
+void download_prop(shard &sh, const prop_host &h, std::size_t pitch, std::size_t off)
+{
+    rows_d2h(sh, h.state, sh.d_state, sh.n_eq, pitch, off);
+    rows_d2h(sh, h.t_hi, sh.d_t_hi, 1u, pitch, off);
+    rows_d2h(sh, h.t_lo, sh.d_t_lo, 1u, pitch, off);
+    rows_d2h(sh, reinterpret_cast<long long *>(h.outcome), sh.d_prop_outcome, 1u, pitch, off);
+    rows_d2h(sh, h.min_h, sh.d_prop_min_h, 1u, pitch, off);
+    rows_d2h(sh, h.max_h, sh.d_prop_max_h, 1u, pitch, off);
+    rows_d2h(sh, reinterpret_cast<unsigned long long *>(h.n_steps), sh.d_prop_n_steps, 1u, pitch, off);
+}
+
+// propagate_until() of every lane of the batch to per-lane final times (host arrays, or device arrays of an unsharded
+// batch: on_device). With io, the shard's slice of the state and times is uploaded before and its results downloaded
+// after its own kernel: the state right away, last_h (and the outcomes, if the iteration limit was hit) once the global
+// exits are known. Returns the flags of the whole batch.
+dev::run_flags propagate(hy_batch *b, const double *tf_hi, const double *tf_lo, const double *mdt, int on_device,
+                         uint64_t max_steps, int write_tc, const prop_host *io)
+{
+    std::vector<prop_ctx> ctx(b->shards.size());
+    for_each_shard(b, [&](shard &sh, std::size_t i) {
+        const std::size_t off = b->off[i];
+        if (io != nullptr) {
+            rows_h2d(sh, sh.d_state, io->state_in, sh.n_eq, b->n, off);
+            rows_h2d(sh, sh.d_pars, io->pars, sh.n_pars, b->n, off);
+            rows_h2d(sh, sh.d_t_hi, io->t_hi_in, 1u, b->n, off);
+            rows_h2d(sh, sh.d_t_lo, io->t_lo_in, 1u, b->n, off);
+        }
+        propagate_phase1(sh, stage(sh, tf_hi, on_device, off, 0), stage(sh, tf_lo, on_device, off, 1),
+                         stage(sh, mdt, on_device, off, 2), max_steps, write_tc, ctx[i]);
+        if (io != nullptr) {
+            download_prop(sh, *io, b->n, off); // (speculative: a non-finite lane anywhere makes every shard run again)
+        }
+    });
+    dev::run_flags ex{0u, 0u, ~0ull, 0ull};
     for (const auto &c : ctx) {
-        any_limit = any_limit || c.fl.any_limit != 0u;
-        loop_len = std::max(loop_len, c.fl.max_iter);
+        if (c.fl.any_nf != 0u) {
+            ex.any_nf = 1u;
+            ex.min_nf_iter = std::min(ex.min_nf_iter, c.fl.min_nf_iter);
+        }
     }
-    for_each_shard(b, [&](hy_batch *sh, std::size_t) { propagate_finish(sh, any_nf, any_limit, loop_len, write_tc); });
-    return HY_OK;
+    if (ex.any_nf != 0u) {
+        // Every lane of every shard stops at the first iteration in which any lane went non-finite.
+        for_each_shard(b, [&](shard &sh, std::size_t i) { propagate_replay(sh, ctx[i], ex.min_nf_iter); });
+    }
+    for (const auto &c : ctx) {
+        ex.any_limit = ex.any_limit != 0u || c.fl.any_limit != 0u ? 1u : 0u;
+        ex.max_iter = std::max(ex.max_iter, c.fl.max_iter);
+    }
+    for_each_shard(b, [&](shard &sh, std::size_t i) {
+        propagate_finish(sh, ex, write_tc);
+        if (io != nullptr) {
+            if (ex.any_nf != 0u || ex.any_limit != 0u) {
+                download_prop(sh, *io, b->n, b->off[i]);
+            }
+            rows_d2h(sh, io->last_h, sh.d_last_h, 1u, b->n, b->off[i]);
+            HY_CUDA_CHECK(cudaStreamSynchronize(sh.stream));
+        }
+    });
+    return ex;
+}
+
+// The device-resident propagations refuse a batch with event equations.
+void refuse_events(const hy_batch *b)
+{
+    if (b != nullptr && b->n_ev != 0u) {
+        throw hy::detail::not_implemented_error("A batch with event equations is propagated by the front end's lock-step "
+                                                "loop over hy_batch_step(), not by the device-resident propagation");
+    }
+}
+
+// The checks of propagate_until_impl() that need the CURRENT times (src/taylor_adaptive_batch.cpp:1212-1273): finite,
+// and final time - current time representable (check_prop_times(): 16 bytes per lane come back from the device for them).
+void check_prop_times_host(std::uint32_t n, const double *t_hi, const double *t_lo, const double *tf_hi, const double *tf_lo)
+{
+    for (std::uint32_t i = 0; i < n; ++i) {
+        if (!std::isfinite(t_hi[i]) || !std::isfinite(t_lo[i])) {
+            throw std::invalid_argument("Cannot invoke the propagate_until() function of an adaptive Taylor integrator "
+                                        "in batch mode if one of the current times is not finite");
+        }
+    }
+    for (std::uint32_t i = 0; i < n; ++i) {
+        // (Same arithmetic as the device: Knuth two-sum of the high parts is enough to detect the overflow.)
+        const double rem = tf_hi[i] - t_hi[i] + ((tf_lo != nullptr ? tf_lo[i] : 0.) - t_lo[i]);
+        if (!std::isfinite(rem)) {
+            throw std::invalid_argument("The final time passed to the propagate_until() function of an adaptive Taylor "
+                                        "integrator in batch mode results in an overflow condition");
+        }
+    }
+}
+
+void check_prop_times(hy_batch *b, const double *tf_hi, const double *tf_lo)
+{
+    std::vector<double> t_hi(b->n), t_lo(b->n);
+    download(b, nullptr, t_hi.data(), t_lo.data(), nullptr);
+    check_prop_times_host(b->n, t_hi.data(), t_lo.data(), tf_hi, tf_lo);
+}
+
+// Argument checks of propagate_until_impl(), src/taylor_adaptive_batch.cpp:1212-1241.
+void check_prop_args(std::uint32_t n, const double *t_final_hi, const double *t_final_lo, const double *max_delta_t)
+{
+    for (std::uint32_t i = 0; i < n; ++i) {
+        if (!std::isfinite(t_final_hi[i]) || (t_final_lo != nullptr && !std::isfinite(t_final_lo[i]))) {
+            throw std::invalid_argument("A non-finite time was passed to the propagate_until() function of an "
+                                        "adaptive Taylor integrator in batch mode");
+        }
+        if (max_delta_t != nullptr) {
+            if (std::isnan(max_delta_t[i])) {
+                throw std::invalid_argument("A nan max_delta_t was passed to the propagate_until() function of an "
+                                            "adaptive Taylor integrator in batch mode");
+            }
+            if (max_delta_t[i] <= 0) {
+                throw std::invalid_argument("A non-positive max_delta_t was passed to the propagate_until() "
+                                            "function of an adaptive Taylor integrator in batch mode");
+            }
+        }
+    }
 }
 
 } // namespace
@@ -1435,7 +1664,6 @@ extern "C" {
 
 int hy_batch_create(const hy_program *p, uint32_t batch, int device, hy_batch **out)
 {
-    hy_batch *b = nullptr;
     try {
         if (p == nullptr || out == nullptr) {
             throw std::invalid_argument("Null pointer passed to hy_batch_create()");
@@ -1443,148 +1671,19 @@ int hy_batch_create(const hy_program *p, uint32_t batch, int device, hy_batch **
         if (batch == 0u) {
             throw std::invalid_argument("The batch size in an adaptive Taylor integrator cannot be zero");
         }
-
         int n_dev = 0;
         if (cudaGetDeviceCount(&n_dev) != cudaSuccess || n_dev == 0) {
             throw cuda_error("No usable CUDA device: heyoka_b200 has no CPU fallback");
         }
-        if (device < 0) {
-            HY_CUDA_CHECK(cudaGetDevice(&device));
-        }
-        if (device >= n_dev) {
-            throw std::invalid_argument("Invalid CUDA device index " + std::to_string(device));
-        }
-
-        // Overflow checks on the buffer sizes, like src/taylor_adaptive_batch.cpp:256-264,375-378.
-        const std::uint64_t tc_size = static_cast<std::uint64_t>(p->n_eq) * (p->order + 1u) * batch;
-        if (tc_size > (std::numeric_limits<std::uint64_t>::max() >> 4)) {
-            throw std::overflow_error("Overflow detected while computing the size of the Taylor coefficients buffer");
-        }
-
-        b = new hy_batch;
-        b->device = device;
-        device_guard guard(device);
-
-        b->n = batch;
-        b->n_eq = p->n_eq;
-        b->n_pars = p->n_pars;
-        b->order = p->order;
-        b->n_uvars = p->n_uvars;
-        b->high_accuracy = p->high_accuracy;
-
-        cudaDeviceProp prop{};
-        HY_CUDA_CHECK(cudaGetDeviceProperties(&prop, device));
-        b->n_sms = static_cast<std::uint32_t>(prop.multiProcessorCount);
-        b->smem_per_block_max = prop.sharedMemPerBlockOptin;
-        b->smem_per_sm = prop.sharedMemPerMultiprocessor;
-
-        // Program arrays, "hbm" encoding.
-        static_assert(sizeof(hy_op) == sizeof(uint4), "hy_op must be 16 bytes");
-        b->d_ops = reinterpret_cast<uint4 *>(b->dupload(p->ops));
-        b->d_args = b->dupload(p->args);
-        b->d_consts = b->dupload(p->consts);
-        b->d_sv_defs = b->dupload(p->sv_defs);
-
-        auto &P = b->prog;
-        P.n_eq = p->n_eq;
-        P.n_uvars = p->n_uvars;
-        P.n_pars = p->n_pars;
-        P.order = p->order;
-        P.n_ops = p->n_uvars - p->n_eq;
-        P.high_accuracy = p->high_accuracy ? 1 : 0;
-        // taylor_determine_h_rhofac(), src/taylor_00.cpp:84-94 (host libm, like the reference's number arithmetic).
-        P.rhofac = std::exp((-7. / 10.) / static_cast<double>(p->order - 1u)) / (std::exp(1.) * std::exp(1.));
-        P.inv_p = 1. / static_cast<double>(p->order);
-        P.inv_pm1 = 1. / static_cast<double>(p->order - 1u);
-        P.ops = b->d_ops;
-        P.args = b->d_args;
-        P.consts = b->d_consts;
-        P.sv_defs = b->d_sv_defs;
-
-        // Cooperative plan.
-        // HEYOKA_B200_FUSE=0 disables the superinstructions, HEYOKA_B200_FUSE_SV=0 the fused state-variable
-        // propagation, HEYOKA_B200_SPILL=0/1 forces the overflow tape off/on (diagnostics / tests).
-        if (const char *env = std::getenv("HEYOKA_B200_FUSE")) {
-            b->opt_fuse = std::string{env} != "0";
-        }
-        if (const char *env = std::getenv("HEYOKA_B200_FUSE_SV")) {
-            b->opt_fuse_sv = std::string{env} != "0";
-        }
-        if (const char *env = std::getenv("HEYOKA_B200_SPILL")) {
-            b->opt_spill = std::string{env} != "0" ? 1 : 0;
-        }
-        if (const char *env = std::getenv("HEYOKA_B200_NB")) {
-            b->opt_nb = std::string{env} != "0" ? 1 : 0;
-        }
-        if (const char *env = std::getenv("HEYOKA_B200_NB_LANE")) {
-            b->opt_nb1 = std::string{env} != "0" ? 1 : 0;
-        }
-        if (const char *env = std::getenv("HEYOKA_B200_NB_THREADS")) {
-            b->opt_nb_threads = static_cast<std::uint32_t>(std::atoi(env));
-        }
-        b->prog_host = std::make_shared<const hy_program>(*p);
-        b->set_tables(b->make_tables(false));
-        b->slab_doubles = static_cast<std::size_t>(p->n_uvars) * (p->order + 1u) * 32u;
-        b->nbp = hy::detail::make_nb_plan(*p);
-        if (const char *env = std::getenv("HEYOKA_B200_NN")) {
-            b->opt_nn = std::string{env} != "0" ? 1 : 0;
-        }
-        b->nnp = hy::detail::make_nn_plan(*p);
-
-        // Resident arrays.
-        const std::size_t n = batch;
-        b->d_state = b->dalloc<double>(n * p->n_eq);
-        b->d_pars = b->dalloc<double>(n * p->n_pars);
-        b->d_t_hi = b->dalloc<double>(n);
-        b->d_t_lo = b->dalloc<double>(n);
-        b->d_last_h = b->dalloc<double>(n);
-        b->d_d_out = b->dalloc<double>(n * p->n_eq);
-        b->d_step_outcome = b->dalloc<long long>(n);
-        b->d_prop_outcome = b->dalloc<long long>(n);
-        b->d_prop_min_h = b->dalloc<double>(n);
-        b->d_prop_max_h = b->dalloc<double>(n);
-        b->d_prop_n_steps = b->dalloc<unsigned long long>(n);
-        b->d_prop_iters = b->dalloc<unsigned long long>(n);
-        b->d_skip = b->dalloc<unsigned char>(n);
-        b->d_tmp = b->dalloc<double>(3u * n);
-        b->d_snapshot = b->dalloc<double>(n * (p->n_eq + 2u));
-        b->d_counter = b->dalloc<unsigned int>(1);
-        b->d_flags = b->dalloc<dev::run_flags>(2); // (+ scratch words behind the flags)
-
-        HY_CUDA_CHECK(cudaMemset(b->d_state, 0, sizeof(double) * n * p->n_eq));
-        HY_CUDA_CHECK(cudaMemset(b->d_pars, 0, sizeof(double) * std::max<std::size_t>(n * p->n_pars, 1u)));
-        HY_CUDA_CHECK(cudaMemset(b->d_t_hi, 0, sizeof(double) * n));
-        HY_CUDA_CHECK(cudaMemset(b->d_t_lo, 0, sizeof(double) * n));
-        HY_CUDA_CHECK(cudaMemset(b->d_last_h, 0, sizeof(double) * n));
-
-        // Kernel selection: HEYOKA_B200_TAPE = hbm | smem overrides the automatic choice.
-        int want = 0;
-        if (const char *env = std::getenv("HEYOKA_B200_TAPE")) {
-            const std::string s{env};
-            want = s == "hbm" ? 1 : (s == "smem" ? 2 : 0);
-        }
-        b->n_ev = static_cast<std::uint32_t>(p->ev_defs.size());
-        if (b->n_ev != 0u) {
-            // Event detection runs on the thread-per-lane kernel family (ev_kernels.cuh).
-            if (p->order + 1u > static_cast<std::uint32_t>(dev::EV_MAXP1)) {
-                throw hy::detail::not_implemented_error("Event detection supports Taylor orders up to "
-                                                        + std::to_string(dev::EV_MAXP1 - 1));
-            }
-            want = 1;
-        }
-        b->commit(b->decide(want, 0, 0, 0, 0));
-
-        *out = b;
+        *out = make_batch(*p, batch, {device}, n_dev, false).release();
         return HY_OK;
     } catch (...) {
-        delete b;
         return translate_exception();
     }
 }
 
 int hy_batch_create_multi(const hy_program *p, uint32_t batch, const int *devices, uint32_t n_devices, hy_batch **out)
 {
-    hy_batch *b = nullptr;
     try {
         if (p == nullptr || out == nullptr) {
             throw std::invalid_argument("Null pointer passed to hy_batch_create_multi()");
@@ -1604,31 +1703,9 @@ int hy_batch_create_multi(const hy_program *p, uint32_t batch, const int *device
         if (batch == 0u) {
             throw std::invalid_argument("The batch size in an adaptive Taylor integrator cannot be zero");
         }
-        // Contiguous blocks of lanes, as even as possible; never more shards than lanes.
-        const std::uint32_t ns = std::min<std::uint32_t>(static_cast<std::uint32_t>(devs.size()), batch);
-        b = new hy_batch;
-        b->n = batch;
-        b->n_eq = p->n_eq;
-        b->n_pars = p->n_pars;
-        b->order = p->order;
-        b->n_uvars = p->n_uvars;
-        b->high_accuracy = p->high_accuracy;
-        b->device = devs[0];
-        b->shard_off.push_back(0u);
-        for (std::uint32_t i = 0; i < ns; ++i) {
-            const std::uint32_t lanes = batch / ns + (i < batch % ns ? 1u : 0u);
-            hy_batch *sh = nullptr;
-            if (hy_batch_create(p, lanes, devs[i], &sh) != HY_OK) {
-                throw std::runtime_error(hy_last_error());
-            }
-            b->shards.push_back(sh);
-            b->shard_off.push_back(b->shard_off.back() + lanes);
-        }
-        b->n_ev = b->shards.empty() ? 0u : b->shards[0]->n_ev; // (event equations: every shard detects its own lanes' events)
-        *out = b;
+        *out = make_batch(*p, batch, devs, n_dev, true).release();
         return HY_OK;
     } catch (...) {
-        delete b;
         return translate_exception();
     }
 }
@@ -1644,7 +1721,7 @@ int hy_device_count(void)
 
 uint32_t hy_batch_n_shards(const hy_batch *b)
 {
-    return b == nullptr ? 0u : static_cast<uint32_t>(b->shards.size());
+    return b == nullptr || !b->multi ? 0u : static_cast<uint32_t>(b->shards.size());
 }
 
 void hy_batch_destroy(hy_batch *b)
@@ -1700,7 +1777,7 @@ int hy_host_unpin(void *ptr)
 
 int hy_batch_set_stream(hy_batch *b, void *cuda_stream)
 {
-    if (b != nullptr && !b->shards.empty()) {
+    if (b != nullptr && b->multi) {
         hy::detail::set_last_error("hy_batch_set_stream() is not available on a multi-device batch");
         return HY_ERR_INVALID_ARG;
     }
@@ -1708,19 +1785,17 @@ int hy_batch_set_stream(hy_batch *b, void *cuda_stream)
         hy::detail::set_last_error("Null batch");
         return HY_ERR_INVALID_ARG;
     }
-    b->stream = static_cast<cudaStream_t>(cuda_stream);
+    b->shards[0]->stream = static_cast<cudaStream_t>(cuda_stream);
     return HY_OK;
 }
 
 int hy_batch_sync(hy_batch *b)
 {
     try {
-        if (!b->shards.empty()) {
-            for_each_shard(b, [](hy_batch *sh, std::size_t) { HY_CUDA_CHECK(cudaStreamSynchronize(sh->stream)); });
-            return HY_OK;
+        if (b == nullptr) {
+            throw std::invalid_argument("Null batch");
         }
-        device_guard guard(b->device);
-        HY_CUDA_CHECK(cudaStreamSynchronize(b->stream));
+        for_each_shard(b, [](shard &sh, std::size_t) { HY_CUDA_CHECK(cudaStreamSynchronize(sh.stream)); });
         return HY_OK;
     } catch (...) {
         return translate_exception();
@@ -1730,20 +1805,19 @@ int hy_batch_sync(hy_batch *b)
 int hy_batch_set_launch_config(hy_batch *b, uint32_t block_threads, uint32_t blocks_per_sm)
 {
     try {
-        if (!b->shards.empty()) {
-            for (auto *sh : b->shards) {
-                if (hy_batch_set_launch_config(sh, block_threads, blocks_per_sm) != HY_OK) {
-                    throw std::runtime_error(hy_last_error());
-                }
-            }
-            return HY_OK;
+        if (b == nullptr) {
+            throw std::invalid_argument("Null batch");
         }
-        device_guard guard(b->device);
-        HY_CUDA_CHECK(cudaStreamSynchronize(b->stream));
-        // The same tape mode and lanes (the N-body kernels derive their lanes per thread from the team; the network
-        // kernel has a fixed shape and ignores every argument).
-        const kernel_sel &k = b->sel;
-        b->commit(b->decide(k.tape_mode, k.L, k.family == kernel_sel::nb ? 0 : k.N, block_threads, blocks_per_sm));
+        // Shard after shard, in shard order: shards on the same device size their scratch from the device memory the
+        // previous shard left free (free_bytes_after_release()).
+        for (auto &sh : b->shards) {
+            device_guard guard(sh->device);
+            HY_CUDA_CHECK(cudaStreamSynchronize(sh->stream));
+            // The same tape mode and lanes (the N-body kernels derive their lanes per thread from the team; the network
+            // kernel has a fixed shape and ignores every argument).
+            const kernel_sel &k = sh->sel;
+            sh->commit(sh->decide(k.tape_mode, k.L, k.family == kernel_sel::nb ? 0 : k.N, block_threads, blocks_per_sm));
+        }
         return HY_OK;
     } catch (...) {
         return translate_exception();
@@ -1760,19 +1834,13 @@ int hy_batch_set_kernel(hy_batch *b, int tape_mode, uint32_t lanes_per_warp, uin
         if (tape_mode < 0 || tape_mode > 9) {
             throw std::invalid_argument("Invalid tape mode");
         }
-        if (!b->shards.empty()) {
-            for (auto *sh : b->shards) {
-                if (hy_batch_set_kernel(sh, tape_mode, lanes_per_warp, lanes_per_thread, block_threads, blocks_per_sm)
-                    != HY_OK) {
-                    throw std::invalid_argument(hy_last_error());
-                }
-            }
-            return HY_OK;
+        // (Shard after shard, in shard order, like hy_batch_set_launch_config().)
+        for (auto &sh : b->shards) {
+            device_guard guard(sh->device);
+            HY_CUDA_CHECK(cudaStreamSynchronize(sh->stream));
+            sh->commit(sh->decide(tape_mode, static_cast<int>(lanes_per_warp), static_cast<int>(lanes_per_thread),
+                                  block_threads, blocks_per_sm));
         }
-        device_guard guard(b->device);
-        HY_CUDA_CHECK(cudaStreamSynchronize(b->stream));
-        b->commit(b->decide(tape_mode, static_cast<int>(lanes_per_warp), static_cast<int>(lanes_per_thread),
-                            block_threads, blocks_per_sm));
         return HY_OK;
     } catch (...) {
         return translate_exception();
@@ -1785,10 +1853,8 @@ int hy_batch_get_kernel(const hy_batch *b, hy_kernel_info *out)
         hy::detail::set_last_error("Null pointer passed to hy_batch_get_kernel()");
         return HY_ERR_INVALID_ARG;
     }
-    if (!b->shards.empty()) {
-        return hy_batch_get_kernel(b->shards[0], out); // (every shard runs the same kernel shape)
-    }
-    const kernel_sel &k = b->sel;
+    const shard &sh = *b->shards[0]; // (every shard runs the same kernel shape)
+    const kernel_sel &k = sh.sel;
     out->tape_mode = k.tape_mode;
     out->lanes_per_warp = static_cast<uint32_t>(k.L);
     out->lanes_per_thread = static_cast<uint32_t>(k.N);
@@ -1797,9 +1863,9 @@ int hy_batch_get_kernel(const hy_batch *b, hy_kernel_info *out)
     out->grid = k.grid;
     out->smem_bytes = k.smem;
     out->tape_slots_per_lane = k.tape_slots;
-    out->n_segments = b->plan.n_segments;
-    out->n_fused = b->plan.n_fused;
-    out->n_sms = b->n_sms;
+    out->n_segments = sh.plan.n_segments;
+    out->n_fused = sh.plan.n_fused;
+    out->n_sms = sh.n_sms;
     out->tmem_cols_per_warp = 0u; // (sm_90 has no tensor memory)
     out->reserved = 0u;
     return HY_OK;
@@ -1808,34 +1874,16 @@ int hy_batch_get_kernel(const hy_batch *b, hy_kernel_info *out)
 int hy_batch_upload(hy_batch *b, const double *state, const double *pars, const double *t_hi, const double *t_lo)
 {
     try {
-        if (!b->shards.empty()) {
-            for_each_shard(b, [&](hy_batch *sh, std::size_t i) {
-                const std::size_t off = b->shard_off[i], n = b->n;
-                rows_h2d(sh, sh->d_state, state, sh->n_eq, n, off);
-                rows_h2d(sh, sh->d_pars, pars, sh->n_pars, n, off);
-                rows_h2d(sh, sh->d_t_hi, t_hi, 1u, n, off);
-                rows_h2d(sh, sh->d_t_lo, t_lo, 1u, n, off);
-                HY_CUDA_CHECK(cudaStreamSynchronize(sh->stream));
-            });
-            return HY_OK;
+        if (b == nullptr) {
+            throw std::invalid_argument("Null batch");
         }
-        device_guard guard(b->device);
-        const std::size_t n = b->n;
-        if (state != nullptr) {
-            HY_CUDA_CHECK(cudaMemcpyAsync(b->d_state, state, sizeof(double) * n * b->n_eq, cudaMemcpyHostToDevice,
-                                          b->stream));
-        }
-        if (pars != nullptr && b->n_pars > 0u) {
-            HY_CUDA_CHECK(cudaMemcpyAsync(b->d_pars, pars, sizeof(double) * n * b->n_pars, cudaMemcpyHostToDevice,
-                                          b->stream));
-        }
-        if (t_hi != nullptr) {
-            HY_CUDA_CHECK(cudaMemcpyAsync(b->d_t_hi, t_hi, sizeof(double) * n, cudaMemcpyHostToDevice, b->stream));
-        }
-        if (t_lo != nullptr) {
-            HY_CUDA_CHECK(cudaMemcpyAsync(b->d_t_lo, t_lo, sizeof(double) * n, cudaMemcpyHostToDevice, b->stream));
-        }
-        HY_CUDA_CHECK(cudaStreamSynchronize(b->stream));
+        for_each_shard(b, [&](shard &sh, std::size_t i) {
+            rows_h2d(sh, sh.d_state, state, sh.n_eq, b->n, b->off[i]);
+            rows_h2d(sh, sh.d_pars, pars, sh.n_pars, b->n, b->off[i]);
+            rows_h2d(sh, sh.d_t_hi, t_hi, 1u, b->n, b->off[i]);
+            rows_h2d(sh, sh.d_t_lo, t_lo, 1u, b->n, b->off[i]);
+            HY_CUDA_CHECK(cudaStreamSynchronize(sh.stream));
+        });
         return HY_OK;
     } catch (...) {
         return translate_exception();
@@ -1845,33 +1893,10 @@ int hy_batch_upload(hy_batch *b, const double *state, const double *pars, const 
 int hy_batch_download(hy_batch *b, double *state, double *t_hi, double *t_lo, double *last_h)
 {
     try {
-        if (!b->shards.empty()) {
-            for_each_shard(b, [&](hy_batch *sh, std::size_t i) {
-                const std::size_t off = b->shard_off[i], n = b->n;
-                rows_d2h(sh, state, sh->d_state, sh->n_eq, n, off);
-                rows_d2h(sh, t_hi, sh->d_t_hi, 1u, n, off);
-                rows_d2h(sh, t_lo, sh->d_t_lo, 1u, n, off);
-                rows_d2h(sh, last_h, sh->d_last_h, 1u, n, off);
-                HY_CUDA_CHECK(cudaStreamSynchronize(sh->stream));
-            });
-            return HY_OK;
+        if (b == nullptr) {
+            throw std::invalid_argument("Null batch");
         }
-        device_guard guard(b->device);
-        const std::size_t n = b->n;
-        if (state != nullptr) {
-            HY_CUDA_CHECK(cudaMemcpyAsync(state, b->d_state, sizeof(double) * n * b->n_eq, cudaMemcpyDeviceToHost,
-                                          b->stream));
-        }
-        if (t_hi != nullptr) {
-            HY_CUDA_CHECK(cudaMemcpyAsync(t_hi, b->d_t_hi, sizeof(double) * n, cudaMemcpyDeviceToHost, b->stream));
-        }
-        if (t_lo != nullptr) {
-            HY_CUDA_CHECK(cudaMemcpyAsync(t_lo, b->d_t_lo, sizeof(double) * n, cudaMemcpyDeviceToHost, b->stream));
-        }
-        if (last_h != nullptr) {
-            HY_CUDA_CHECK(cudaMemcpyAsync(last_h, b->d_last_h, sizeof(double) * n, cudaMemcpyDeviceToHost, b->stream));
-        }
-        HY_CUDA_CHECK(cudaStreamSynchronize(b->stream));
+        download(b, state, t_hi, t_lo, last_h);
         return HY_OK;
     } catch (...) {
         return translate_exception();
@@ -1881,25 +1906,14 @@ int hy_batch_download(hy_batch *b, double *state, double *t_hi, double *t_lo, do
 int hy_batch_download_step_res(hy_batch *b, int64_t *outcome, double *h)
 {
     try {
-        if (!b->shards.empty()) {
-            for_each_shard(b, [&](hy_batch *sh, std::size_t i) {
-                const std::size_t off = b->shard_off[i], n = b->n;
-                rows_d2h(sh, reinterpret_cast<long long *>(outcome), sh->d_step_outcome, 1u, n, off);
-                rows_d2h(sh, h, sh->d_last_h, 1u, n, off);
-                HY_CUDA_CHECK(cudaStreamSynchronize(sh->stream));
-            });
-            return HY_OK;
+        if (b == nullptr) {
+            throw std::invalid_argument("Null batch");
         }
-        device_guard guard(b->device);
-        const std::size_t n = b->n;
-        if (outcome != nullptr) {
-            HY_CUDA_CHECK(cudaMemcpyAsync(outcome, b->d_step_outcome, sizeof(int64_t) * n, cudaMemcpyDeviceToHost,
-                                          b->stream));
-        }
-        if (h != nullptr) {
-            HY_CUDA_CHECK(cudaMemcpyAsync(h, b->d_last_h, sizeof(double) * n, cudaMemcpyDeviceToHost, b->stream));
-        }
-        HY_CUDA_CHECK(cudaStreamSynchronize(b->stream));
+        for_each_shard(b, [&](shard &sh, std::size_t i) {
+            rows_d2h(sh, reinterpret_cast<long long *>(outcome), sh.d_step_outcome, 1u, b->n, b->off[i]);
+            rows_d2h(sh, h, sh.d_last_h, 1u, b->n, b->off[i]);
+            HY_CUDA_CHECK(cudaStreamSynchronize(sh.stream));
+        });
         return HY_OK;
     } catch (...) {
         return translate_exception();
@@ -1909,36 +1923,16 @@ int hy_batch_download_step_res(hy_batch *b, int64_t *outcome, double *h)
 int hy_batch_download_prop_res(hy_batch *b, int64_t *outcome, double *min_h, double *max_h, uint64_t *n_steps)
 {
     try {
-        if (!b->shards.empty()) {
-            for_each_shard(b, [&](hy_batch *sh, std::size_t i) {
-                const std::size_t off = b->shard_off[i], n = b->n;
-                rows_d2h(sh, reinterpret_cast<long long *>(outcome), sh->d_prop_outcome, 1u, n, off);
-                rows_d2h(sh, min_h, sh->d_prop_min_h, 1u, n, off);
-                rows_d2h(sh, max_h, sh->d_prop_max_h, 1u, n, off);
-                rows_d2h(sh, reinterpret_cast<unsigned long long *>(n_steps), sh->d_prop_n_steps, 1u, n, off);
-                HY_CUDA_CHECK(cudaStreamSynchronize(sh->stream));
-            });
-            return HY_OK;
+        if (b == nullptr) {
+            throw std::invalid_argument("Null batch");
         }
-        device_guard guard(b->device);
-        const std::size_t n = b->n;
-        if (outcome != nullptr) {
-            HY_CUDA_CHECK(cudaMemcpyAsync(outcome, b->d_prop_outcome, sizeof(int64_t) * n, cudaMemcpyDeviceToHost,
-                                          b->stream));
-        }
-        if (min_h != nullptr) {
-            HY_CUDA_CHECK(cudaMemcpyAsync(min_h, b->d_prop_min_h, sizeof(double) * n, cudaMemcpyDeviceToHost,
-                                          b->stream));
-        }
-        if (max_h != nullptr) {
-            HY_CUDA_CHECK(cudaMemcpyAsync(max_h, b->d_prop_max_h, sizeof(double) * n, cudaMemcpyDeviceToHost,
-                                          b->stream));
-        }
-        if (n_steps != nullptr) {
-            HY_CUDA_CHECK(cudaMemcpyAsync(n_steps, b->d_prop_n_steps, sizeof(uint64_t) * n, cudaMemcpyDeviceToHost,
-                                          b->stream));
-        }
-        HY_CUDA_CHECK(cudaStreamSynchronize(b->stream));
+        for_each_shard(b, [&](shard &sh, std::size_t i) {
+            rows_d2h(sh, reinterpret_cast<long long *>(outcome), sh.d_prop_outcome, 1u, b->n, b->off[i]);
+            rows_d2h(sh, min_h, sh.d_prop_min_h, 1u, b->n, b->off[i]);
+            rows_d2h(sh, max_h, sh.d_prop_max_h, 1u, b->n, b->off[i]);
+            rows_d2h(sh, reinterpret_cast<unsigned long long *>(n_steps), sh.d_prop_n_steps, 1u, b->n, b->off[i]);
+            HY_CUDA_CHECK(cudaStreamSynchronize(sh.stream));
+        });
         return HY_OK;
     } catch (...) {
         return translate_exception();
@@ -1948,19 +1942,14 @@ int hy_batch_download_prop_res(hy_batch *b, int64_t *outcome, double *min_h, dou
 int hy_batch_download_tc(hy_batch *b, double *tc)
 {
     try {
-        if (!b->shards.empty()) {
-            for_each_shard(b, [&](hy_batch *sh, std::size_t i) {
-                sh->ensure_tc();
-                rows_d2h(sh, tc, sh->d_tc, static_cast<std::size_t>(sh->n_eq) * (sh->order + 1u), b->n, b->shard_off[i]);
-                HY_CUDA_CHECK(cudaStreamSynchronize(sh->stream));
-            });
-            return HY_OK;
+        if (b == nullptr) {
+            throw std::invalid_argument("Null batch");
         }
-        device_guard guard(b->device);
-        const std::size_t sz = static_cast<std::size_t>(b->n_eq) * (b->order + 1u) * b->n;
-        b->ensure_tc();
-        HY_CUDA_CHECK(cudaMemcpyAsync(tc, b->d_tc, sizeof(double) * sz, cudaMemcpyDeviceToHost, b->stream));
-        HY_CUDA_CHECK(cudaStreamSynchronize(b->stream));
+        for_each_shard(b, [&](shard &sh, std::size_t i) {
+            sh.ensure_tc();
+            rows_d2h(sh, tc, sh.d_tc, static_cast<std::size_t>(sh.n_eq) * (sh.order + 1u), b->n, b->off[i]);
+            HY_CUDA_CHECK(cudaStreamSynchronize(sh.stream));
+        });
         return HY_OK;
     } catch (...) {
         return translate_exception();
@@ -1973,19 +1962,11 @@ int hy_batch_upload_tc(hy_batch *b, const double *tc)
         if (b == nullptr || tc == nullptr) {
             throw std::invalid_argument("Null pointer passed to hy_batch_upload_tc()");
         }
-        if (!b->shards.empty()) {
-            for_each_shard(b, [&](hy_batch *sh, std::size_t i) {
-                sh->ensure_tc();
-                rows_h2d(sh, sh->d_tc, tc, static_cast<std::size_t>(sh->n_eq) * (sh->order + 1u), b->n, b->shard_off[i]);
-                HY_CUDA_CHECK(cudaStreamSynchronize(sh->stream));
-            });
-            return HY_OK;
-        }
-        device_guard guard(b->device);
-        b->ensure_tc();
-        const std::size_t sz = static_cast<std::size_t>(b->n_eq) * (b->order + 1u) * b->n;
-        HY_CUDA_CHECK(cudaMemcpyAsync(b->d_tc, tc, sizeof(double) * sz, cudaMemcpyHostToDevice, b->stream));
-        HY_CUDA_CHECK(cudaStreamSynchronize(b->stream));
+        for_each_shard(b, [&](shard &sh, std::size_t i) {
+            sh.ensure_tc();
+            rows_h2d(sh, sh.d_tc, tc, static_cast<std::size_t>(sh.n_eq) * (sh.order + 1u), b->n, b->off[i]);
+            HY_CUDA_CHECK(cudaStreamSynchronize(sh.stream));
+        });
         return HY_OK;
     } catch (...) {
         return translate_exception();
@@ -1994,7 +1975,7 @@ int hy_batch_upload_tc(hy_batch *b, const double *tc)
 
 int hy_batch_get_ptrs(hy_batch *b, hy_batch_ptrs *out)
 {
-    if (b != nullptr && !b->shards.empty()) {
+    if (b != nullptr && b->multi) {
         hy::detail::set_last_error("hy_batch_get_ptrs() is not available on a multi-device batch: use the shards");
         return HY_ERR_INVALID_ARG;
     }
@@ -2002,49 +1983,31 @@ int hy_batch_get_ptrs(hy_batch *b, hy_batch_ptrs *out)
         hy::detail::set_last_error("Null pointer passed to hy_batch_get_ptrs()");
         return HY_ERR_INVALID_ARG;
     }
-    out->state = b->d_state;
-    out->pars = b->d_pars;
-    out->t_hi = b->d_t_hi;
-    out->t_lo = b->d_t_lo;
-    out->last_h = b->d_last_h;
-    out->tc = b->d_tc; // null until a step with write_tc / a dense output has been requested
-    out->d_out = b->d_d_out;
-    out->step_outcome = reinterpret_cast<int64_t *>(b->d_step_outcome);
-    out->prop_outcome = reinterpret_cast<int64_t *>(b->d_prop_outcome);
-    out->prop_min_h = b->d_prop_min_h;
-    out->prop_max_h = b->d_prop_max_h;
-    out->prop_n_steps = reinterpret_cast<uint64_t *>(b->d_prop_n_steps);
+    const shard &sh = *b->shards[0];
+    out->state = sh.d_state;
+    out->pars = sh.d_pars;
+    out->t_hi = sh.d_t_hi;
+    out->t_lo = sh.d_t_lo;
+    out->last_h = sh.d_last_h;
+    out->tc = sh.d_tc; // null until a step with write_tc / a dense output has been requested
+    out->d_out = sh.d_d_out;
+    out->step_outcome = reinterpret_cast<int64_t *>(sh.d_step_outcome);
+    out->prop_outcome = reinterpret_cast<int64_t *>(sh.d_prop_outcome);
+    out->prop_min_h = sh.d_prop_min_h;
+    out->prop_max_h = sh.d_prop_max_h;
+    out->prop_n_steps = reinterpret_cast<uint64_t *>(sh.d_prop_n_steps);
     return HY_OK;
 }
 
 int hy_batch_step(hy_batch *b, const double *max_delta_t, int on_device, int backward, int write_tc)
 {
     try {
-        if (!b->shards.empty()) {
-            if (on_device) {
-                throw std::invalid_argument("Device-resident step limits are not available on a multi-device batch");
-            }
-            for_each_shard(b, [&](hy_batch *sh, std::size_t i) {
-                if (hy_batch_step(sh, max_delta_t != nullptr ? max_delta_t + b->shard_off[i] : nullptr, 0, backward,
-                                  write_tc)
-                    != HY_OK) {
-                    throw std::invalid_argument(hy_last_error());
-                }
-            });
-            if (b->n_ev != 0u) {
-                // The events of the step, lanes ascending like on one device: the shards' lists one after the other,
-                // with the lanes of the whole batch.
-                b->ev_host.clear();
-                for (std::size_t i = 0; i < b->shards.size(); ++i) {
-                    for (hy_event_rec r : b->shards[i]->ev_host) {
-                        r.lane += b->shard_off[i];
-                        b->ev_host.push_back(r);
-                    }
-                }
-            }
-            return HY_OK;
+        if (b == nullptr) {
+            throw std::invalid_argument("Null batch");
         }
-        device_guard guard(b->device);
+        if (on_device && b->multi) {
+            throw std::invalid_argument("Device-resident step limits are not available on a multi-device batch");
+        }
         if (max_delta_t != nullptr && !on_device) {
             // step(max_delta_ts): NaN limits are rejected (src/taylor_adaptive_batch.cpp:1060-1075).
             for (std::uint32_t i = 0; i < b->n; ++i) {
@@ -2054,114 +2017,69 @@ int hy_batch_step(hy_batch *b, const double *max_delta_t, int on_device, int bac
                 }
             }
         }
-        if (b->n_ev != 0u) {
-            // A batch with event equations: every step detects events (the Taylor coefficients are always written,
-            // src/taylor_adaptive_batch.cpp:776); hy_batch_get_events() returns what was found.
-            b->ev_step(stage(b, max_delta_t, on_device, 0), on_device, backward);
-            return HY_OK;
+        if (b->n_ev != 0u && !b->ev_set) {
+            throw std::invalid_argument("hy_batch_set_events() must be called before stepping a batch with event equations");
         }
-        dev::run_args R{};
-        R.max_delta_t = stage(b, max_delta_t, on_device, 0);
-        R.default_max_delta_t
-            = backward ? -std::numeric_limits<double>::infinity() : std::numeric_limits<double>::infinity();
-        R.write_tc = write_tc;
-        R.flags = b->d_flags;
-        R.counter = b->d_counter;
-        b->launch(false, R);
+        std::vector<std::vector<hy_event_rec>> evs(b->shards.size());
+        for_each_shard(b, [&](shard &sh, std::size_t i) {
+            const double *d_mdt = stage(sh, max_delta_t, on_device, b->off[i], 0);
+            if (b->n_ev != 0u) {
+                // A batch with event equations: every step detects events (the Taylor coefficients are always written,
+                // src/taylor_adaptive_batch.cpp:776); hy_batch_get_events() returns what was found.
+                evs[i] = sh.ev_step(d_mdt, backward);
+                return;
+            }
+            dev::run_args R{};
+            R.max_delta_t = d_mdt;
+            R.default_max_delta_t
+                = backward ? -std::numeric_limits<double>::infinity() : std::numeric_limits<double>::infinity();
+            R.write_tc = write_tc;
+            R.flags = sh.d_flags;
+            R.counter = sh.d_counter;
+            sh.launch(false, R);
+        });
+        if (b->n_ev != 0u) {
+            // The shards' lists one after the other, with the lanes of the whole batch: lanes ascending.
+            b->ev_host.clear();
+            for (std::size_t i = 0; i < evs.size(); ++i) {
+                for (hy_event_rec r : evs[i]) {
+                    r.lane += b->off[i];
+                    b->ev_host.push_back(r);
+                }
+            }
+        }
         return HY_OK;
     } catch (...) {
         return translate_exception();
     }
 }
 
-namespace
-{
-
-// The checks of propagate_until_impl() that need the CURRENT times (src/taylor_adaptive_batch.cpp:1212-1273): finite,
-// and final time - current time representable (check_prop_times(): 16 bytes per lane come back from the device for them).
-void check_prop_times_host(std::uint32_t n, const double *t_hi, const double *t_lo, const double *tf_hi, const double *tf_lo)
-{
-    for (std::uint32_t i = 0; i < n; ++i) {
-        if (!std::isfinite(t_hi[i]) || !std::isfinite(t_lo[i])) {
-            throw std::invalid_argument("Cannot invoke the propagate_until() function of an adaptive Taylor integrator "
-                                        "in batch mode if one of the current times is not finite");
-        }
-    }
-    for (std::uint32_t i = 0; i < n; ++i) {
-        // (Same arithmetic as the device: Knuth two-sum of the high parts is enough to detect the overflow.)
-        const double rem = tf_hi[i] - t_hi[i] + ((tf_lo != nullptr ? tf_lo[i] : 0.) - t_lo[i]);
-        if (!std::isfinite(rem)) {
-            throw std::invalid_argument("The final time passed to the propagate_until() function of an adaptive Taylor "
-                                        "integrator in batch mode results in an overflow condition");
-        }
-    }
-}
-
-void check_prop_times(hy_batch *b, const double *tf_hi, const double *tf_lo)
-{
-    std::vector<double> t_hi(b->n), t_lo(b->n);
-    if (hy_batch_download(b, nullptr, t_hi.data(), t_lo.data(), nullptr) != HY_OK) {
-        throw cuda_error(hy_last_error());
-    }
-    check_prop_times_host(b->n, t_hi.data(), t_lo.data(), tf_hi, tf_lo);
-}
-
-// Argument checks of propagate_until_impl(), src/taylor_adaptive_batch.cpp:1212-1241.
-void check_prop_args(std::uint32_t n, const double *t_final_hi, const double *t_final_lo, const double *max_delta_t)
-{
-    for (std::uint32_t i = 0; i < n; ++i) {
-        if (!std::isfinite(t_final_hi[i]) || (t_final_lo != nullptr && !std::isfinite(t_final_lo[i]))) {
-            throw std::invalid_argument("A non-finite time was passed to the propagate_until() function of an "
-                                        "adaptive Taylor integrator in batch mode");
-        }
-        if (max_delta_t != nullptr) {
-            if (std::isnan(max_delta_t[i])) {
-                throw std::invalid_argument("A nan max_delta_t was passed to the propagate_until() function of an "
-                                            "adaptive Taylor integrator in batch mode");
-            }
-            if (max_delta_t[i] <= 0) {
-                throw std::invalid_argument("A non-positive max_delta_t was passed to the propagate_until() "
-                                            "function of an adaptive Taylor integrator in batch mode");
-            }
-        }
-    }
-}
-
-} // namespace
-
 int hy_batch_propagate_until(hy_batch *b, const double *t_final_hi, const double *t_final_lo, const double *max_delta_t,
                              uint64_t max_steps, int write_tc)
 {
     try {
-        if (b != nullptr && b->n_ev != 0u) {
-            throw hy::detail::not_implemented_error("A batch with event equations is propagated by the front end's lock-step "
-                                                    "loop over hy_batch_step(), not by the device-resident propagation");
+        refuse_events(b);
+        if (b == nullptr) {
+            throw std::invalid_argument("Null batch");
         }
-        device_guard guard(b->device);
         if (t_final_hi == nullptr) {
             throw std::invalid_argument("Null final times passed to hy_batch_propagate_until()");
         }
         check_prop_args(b->n, t_final_hi, t_final_lo, max_delta_t);
         check_prop_times(b, t_final_hi, t_final_lo);
-        if (!b->shards.empty()) {
-            return multi_propagate(b, t_final_hi, t_final_lo, max_delta_t, max_steps, write_tc);
-        }
-        const double *d_hi = stage(b, t_final_hi, 0, 0);
-        const double *d_lo = stage(b, t_final_lo, 0, 1);
-        const double *d_mdt = stage(b, max_delta_t, 0, 2);
-        return propagate_impl(b, d_hi, d_lo, d_mdt, max_steps, write_tc, nullptr);
+        propagate(b, t_final_hi, t_final_lo, max_delta_t, 0, max_steps, write_tc, nullptr);
+        return HY_OK;
     } catch (...) {
         return translate_exception();
     }
 }
 
 // propagate_until() on HOST buffers in one call: upload of state / parameters / times, propagation, download of state,
-// times, last_h and the per-lane results (the outputs may alias the inputs). On a batch made of shards (hy_batch_create_multi(): several devices, or the
-// SAME device listed several times) every shard runs its copies and its kernel on its own stream from its own host
-// thread: with k shards on one device the copies of a shard overlap the kernels of the others, and only 1 / k of the
-// transfers stays exposed. The checks on the current times are done on the caller's arrays (no read-back), the state is
-// downloaded right after the shard's kernel; only last_h (and the outcomes, if the iteration limit was hit) wait for the
-// global exits across the shards.
+// times, last_h and the per-lane results (the outputs may alias the inputs). On a batch made of shards
+// (hy_batch_create_multi(): several devices, or the SAME device listed several times) every shard runs its copies and
+// its kernel on its own stream from its own host thread: with k shards on one device the copies of a shard overlap the
+// kernels of the others, and only 1 / k of the transfers stays exposed. The checks on the current times are done on the
+// caller's arrays (no read-back).
 int hy_batch_propagate_until_host(hy_batch *b, const double *state_in, const double *pars, const double *t_hi_in,
                                   const double *t_lo_in, const double *t_final_hi, const double *t_final_lo,
                                   const double *max_delta_t, uint64_t max_steps, double *state, double *t_hi, double *t_lo,
@@ -2171,73 +2089,11 @@ int hy_batch_propagate_until_host(hy_batch *b, const double *state_in, const dou
         if (b == nullptr || state_in == nullptr || t_hi_in == nullptr || t_lo_in == nullptr || t_final_hi == nullptr) {
             throw std::invalid_argument("Null pointer passed to hy_batch_propagate_until_host()");
         }
-        if (b->n_ev != 0u) {
-            throw hy::detail::not_implemented_error("A batch with event equations is propagated by the front end's lock-step "
-                                                    "loop over hy_batch_step(), not by the device-resident propagation");
-        }
-        device_guard guard(b->device);
+        refuse_events(b);
         check_prop_args(b->n, t_final_hi, t_final_lo, max_delta_t);
         check_prop_times_host(b->n, t_hi_in, t_lo_in, t_final_hi, t_final_lo);
-        const bool multi = !b->shards.empty();
-        const std::size_t ns = multi ? b->shards.size() : 1u, pitch = b->n;
-        std::vector<prop_ctx> ctx(ns);
-        const auto offset = [&](std::size_t i) { return multi ? static_cast<std::size_t>(b->shard_off[i]) : std::size_t(0); };
-        const auto each = [&](auto &&fn) {
-            if (multi) {
-                for_each_shard(b, fn);
-            } else {
-                fn(b, std::size_t(0));
-            }
-        };
-        const auto download_main = [&](hy_batch *sh, std::size_t off) {
-            rows_d2h(sh, state, sh->d_state, sh->n_eq, pitch, off);
-            rows_d2h(sh, t_hi, sh->d_t_hi, 1u, pitch, off);
-            rows_d2h(sh, t_lo, sh->d_t_lo, 1u, pitch, off);
-            rows_d2h(sh, reinterpret_cast<long long *>(outcome), sh->d_prop_outcome, 1u, pitch, off);
-            rows_d2h(sh, min_h, sh->d_prop_min_h, 1u, pitch, off);
-            rows_d2h(sh, max_h, sh->d_prop_max_h, 1u, pitch, off);
-            rows_d2h(sh, reinterpret_cast<unsigned long long *>(n_steps), sh->d_prop_n_steps, 1u, pitch, off);
-        };
-        each([&](hy_batch *sh, std::size_t i) {
-            const std::size_t off = offset(i);
-            rows_h2d(sh, sh->d_state, state_in, sh->n_eq, pitch, off);
-            rows_h2d(sh, sh->d_pars, pars, sh->n_pars, pitch, off);
-            rows_h2d(sh, sh->d_t_hi, t_hi_in, 1u, pitch, off);
-            rows_h2d(sh, sh->d_t_lo, t_lo_in, 1u, pitch, off);
-            const double *d_hi = stage(sh, t_final_hi + off, 0, 0);
-            const double *d_lo = stage(sh, t_final_lo != nullptr ? t_final_lo + off : nullptr, 0, 1);
-            const double *d_mdt = stage(sh, max_delta_t != nullptr ? max_delta_t + off : nullptr, 0, 2);
-            propagate_phase1(sh, d_hi, d_lo, d_mdt, max_steps, 0, ctx[i]);
-            // (Speculative: a non-finite lane anywhere makes every shard run again, see below.)
-            download_main(sh, off);
-        });
-        bool any_nf = false, any_limit = false;
-        unsigned long long cap = ~0ull, loop_len = 0;
-        for (const auto &c : ctx) {
-            if (c.fl.any_nf != 0u) {
-                any_nf = true;
-                cap = std::min(cap, c.fl.min_nf_iter);
-            }
-        }
-        if (any_nf) {
-            each([&](hy_batch *sh, std::size_t i) {
-                HY_CUDA_CHECK(cudaStreamSynchronize(sh->stream));
-                propagate_replay(sh, ctx[i], cap);
-            });
-        }
-        for (const auto &c : ctx) {
-            any_limit = any_limit || c.fl.any_limit != 0u;
-            loop_len = std::max(loop_len, c.fl.max_iter);
-        }
-        each([&](hy_batch *sh, std::size_t i) {
-            const std::size_t off = offset(i);
-            propagate_finish(sh, any_nf, any_limit, loop_len, 0);
-            if (any_nf || any_limit) {
-                download_main(sh, off);
-            }
-            rows_d2h(sh, last_h, sh->d_last_h, 1u, pitch, off);
-            HY_CUDA_CHECK(cudaStreamSynchronize(sh->stream));
-        });
+        const prop_host io{state_in, pars, t_hi_in, t_lo_in, state, t_hi, t_lo, last_h, outcome, min_h, max_h, n_steps};
+        propagate(b, t_final_hi, t_final_lo, max_delta_t, 0, max_steps, 0, &io);
         return HY_OK;
     } catch (...) {
         return translate_exception();
@@ -2248,18 +2104,21 @@ int hy_batch_propagate_until_dev(hy_batch *b, const double *d_t_final_hi, const 
                                  const double *d_max_delta_t, uint64_t max_steps, int write_tc, int *any_nf_or_limit)
 {
     try {
-        if (b != nullptr && b->n_ev != 0u) {
-            throw hy::detail::not_implemented_error("A batch with event equations is propagated by the front end's lock-step "
-                                                    "loop over hy_batch_step(), not by the device-resident propagation");
+        refuse_events(b);
+        if (b == nullptr) {
+            throw std::invalid_argument("Null batch");
         }
-        if (!b->shards.empty()) {
+        if (b->multi) {
             throw std::invalid_argument("hy_batch_propagate_until_dev() is not available on a multi-device batch");
         }
-        device_guard guard(b->device);
         if (d_t_final_hi == nullptr) {
             throw std::invalid_argument("Null final times passed to hy_batch_propagate_until_dev()");
         }
-        return propagate_impl(b, d_t_final_hi, d_t_final_lo, d_max_delta_t, max_steps, write_tc, any_nf_or_limit);
+        const dev::run_flags ex = propagate(b, d_t_final_hi, d_t_final_lo, d_max_delta_t, 1, max_steps, write_tc, nullptr);
+        if (any_nf_or_limit != nullptr) {
+            *any_nf_or_limit = (ex.any_nf != 0u ? 1 : 0) | (ex.any_limit != 0u ? 2 : 0);
+        }
+        return HY_OK;
     } catch (...) {
         return translate_exception();
     }
@@ -2285,16 +2144,11 @@ void check_grid(hy_batch *b, const double *grid, uint64_t n_pts, const double *m
     }
     // The current time must be finite (:1590-1594).
     std::vector<double> t_hi(n), t_lo(n);
-    {
-        // (Through the download entry point: it also serves a batch made of shards.)
-        if (hy_batch_download(b, nullptr, t_hi.data(), t_lo.data(), nullptr) != HY_OK) {
-            throw cuda_error(hy_last_error());
-        }
-        for (std::uint32_t i = 0; i < n; ++i) {
-            if (!std::isfinite(t_hi[i]) || !std::isfinite(t_lo[i])) {
-                throw std::invalid_argument("Cannot invoke propagate_grid() in an adaptive Taylor integrator in "
-                                            "batch mode if the current time is not finite");
-            }
+    download(b, nullptr, t_hi.data(), t_lo.data(), nullptr);
+    for (std::uint32_t i = 0; i < n; ++i) {
+        if (!std::isfinite(t_hi[i]) || !std::isfinite(t_lo[i])) {
+            throw std::invalid_argument("Cannot invoke propagate_grid() in an adaptive Taylor integrator in "
+                                        "batch mode if the current time is not finite");
         }
     }
     if (max_delta_t != nullptr) {
@@ -2360,7 +2214,6 @@ int hy_batch_check_grid(hy_batch *b, const double *grid, uint64_t n_pts, const d
         if (b == nullptr || grid == nullptr) {
             throw std::invalid_argument("Null pointer passed to hy_batch_check_grid()");
         }
-        device_guard guard(b->device);
         check_grid(b, grid, n_pts, max_delta_t);
         return HY_OK;
     } catch (...) {
@@ -2384,39 +2237,37 @@ int hy_batch_propagate_grid(hy_batch *b, const double *grid, uint64_t n_pts, con
         }
     };
     try {
-        if (b != nullptr && b->n_ev != 0u) {
-            throw hy::detail::not_implemented_error("A batch with event equations is propagated by the front end's lock-step "
-                                                    "loop over hy_batch_step(), not by the device-resident propagation");
-        }
+        refuse_events(b);
         if (b == nullptr || grid == nullptr || out == nullptr) {
             throw std::invalid_argument("Null pointer passed to hy_batch_propagate_grid()");
         }
-        if (!b->shards.empty()) {
+        if (b->multi) {
             throw hy::detail::not_implemented_error("propagate_grid() is not available on a multi-device batch");
         }
-        device_guard guard(b->device);
-        const std::uint32_t n = b->n;
         check_grid(b, grid, n_pts, max_delta_t);
+        shard &sh = *b->shards[0];
+        device_guard guard(sh.device);
+        const std::uint32_t n = sh.n;
 
-        const std::size_t n_out = static_cast<std::size_t>(n_pts) * b->n_eq * n, state_doubles = std::size_t(b->n_eq) * n;
+        const std::size_t n_out = static_cast<std::size_t>(n_pts) * sh.n_eq * n, state_doubles = std::size_t(sh.n_eq) * n;
         HY_CUDA_CHECK(cudaMalloc(&d_grid, sizeof(double) * n_pts * n));
         HY_CUDA_CHECK(cudaMalloc(&d_out, sizeof(double) * n_out));
         HY_CUDA_CHECK(cudaMalloc(&d_lane, sizeof(double) * 4u * n)); // rem_hi, rem_lo, dt_limit, max_delta_t
         HY_CUDA_CHECK(cudaMalloc(&d_idx, sizeof(std::uint32_t) * n));
         HY_CUDA_CHECK(cudaMalloc(&d_dir, n));
         HY_CUDA_CHECK(cudaMalloc(&d_gflags, sizeof(unsigned) * 4u));
-        HY_CUDA_CHECK(cudaMemcpyAsync(d_grid, grid, sizeof(double) * n_pts * n, cudaMemcpyHostToDevice, b->stream));
+        HY_CUDA_CHECK(cudaMemcpyAsync(d_grid, grid, sizeof(double) * n_pts * n, cudaMemcpyHostToDevice, sh.stream));
         if (max_delta_t != nullptr) {
             HY_CUDA_CHECK(cudaMemcpyAsync(d_lane + 3u * n, max_delta_t, sizeof(double) * n, cudaMemcpyHostToDevice,
-                                          b->stream));
+                                          sh.stream));
         }
-        dev::k_fill_double<<<static_cast<unsigned>((n_out + 255u) / 256u), 256, 0, b->stream>>>(
+        dev::k_fill_double<<<static_cast<unsigned>((n_out + 255u) / 256u), 256, 0, sh.stream>>>(
             d_out, n_out, std::numeric_limits<double>::quiet_NaN());
         HY_CUDA_CHECK(cudaGetLastError());
         const unsigned gb = (n + 127u) / 128u;
         const auto finish = [&]() {
-            HY_CUDA_CHECK(cudaMemcpyAsync(out, d_out, sizeof(double) * n_out, cudaMemcpyDeviceToHost, b->stream));
-            HY_CUDA_CHECK(cudaStreamSynchronize(b->stream));
+            HY_CUDA_CHECK(cudaMemcpyAsync(out, d_out, sizeof(double) * n_out, cudaMemcpyDeviceToHost, sh.stream));
+            HY_CUDA_CHECK(cudaStreamSynchronize(sh.stream));
             cleanup();
             return HY_OK;
         };
@@ -2424,26 +2275,21 @@ int hy_batch_propagate_grid(hy_batch *b, const double *grid, uint64_t n_pts, con
         // Up to the first grid point (a zero-length step when the time is already there: it brings the Taylor
         // coefficients up to date), :1697-1706.
         {
-            const double *d_mdt = max_delta_t != nullptr ? d_lane + 3u * n : nullptr;
-            const int rc = propagate_impl(b, d_grid, nullptr, d_mdt, max_steps, 1, nullptr);
-            if (rc != HY_OK) {
-                cleanup();
-                return rc;
-            }
+            propagate(b, d_grid, nullptr, max_delta_t != nullptr ? d_lane + 3u * n : nullptr, 1, max_steps, 1, nullptr);
             std::vector<long long> oc(n);
-            HY_CUDA_CHECK(cudaMemcpyAsync(oc.data(), b->d_prop_outcome, sizeof(long long) * n, cudaMemcpyDeviceToHost,
-                                          b->stream));
-            HY_CUDA_CHECK(cudaStreamSynchronize(b->stream));
+            HY_CUDA_CHECK(cudaMemcpyAsync(oc.data(), sh.d_prop_outcome, sizeof(long long) * n, cudaMemcpyDeviceToHost,
+                                          sh.stream));
+            HY_CUDA_CHECK(cudaStreamSynchronize(sh.stream));
             if (std::any_of(oc.begin(), oc.end(), [](long long v) { return v != HY_OUTCOME_TIME_LIMIT; })) {
                 // Outcomes kept, counters reset (:1709-1722).
-                dev::k_fill_double<<<gb, 128, 0, b->stream>>>(b->d_prop_min_h, n, std::numeric_limits<double>::infinity());
-                dev::k_fill_double<<<gb, 128, 0, b->stream>>>(b->d_prop_max_h, n, 0.);
-                HY_CUDA_CHECK(cudaMemsetAsync(b->d_prop_n_steps, 0, sizeof(unsigned long long) * n, b->stream));
+                dev::k_fill_double<<<gb, 128, 0, sh.stream>>>(sh.d_prop_min_h, n, std::numeric_limits<double>::infinity());
+                dev::k_fill_double<<<gb, 128, 0, sh.stream>>>(sh.d_prop_max_h, n, 0.);
+                HY_CUDA_CHECK(cudaMemsetAsync(sh.d_prop_n_steps, 0, sizeof(unsigned long long) * n, sh.stream));
                 return finish();
             }
         }
-        HY_CUDA_CHECK(cudaMemcpyAsync(d_out, b->d_state, sizeof(double) * state_doubles, cudaMemcpyDeviceToDevice,
-                                      b->stream));
+        HY_CUDA_CHECK(cudaMemcpyAsync(d_out, sh.d_state, sizeof(double) * state_doubles, cudaMemcpyDeviceToDevice,
+                                      sh.stream));
 
         dev::grid_state G{};
         G.grid = d_grid;
@@ -2458,13 +2304,13 @@ int hy_batch_propagate_grid(hy_batch *b, const double *grid, uint64_t n_pts, con
         G.flags = d_gflags;
         unsigned hflags[4] = {0u, 0u, 0u, 0u};
         const auto read_flags = [&]() {
-            HY_CUDA_CHECK(cudaMemcpyAsync(hflags, d_gflags, sizeof(hflags), cudaMemcpyDeviceToHost, b->stream));
-            HY_CUDA_CHECK(cudaStreamSynchronize(b->stream));
+            HY_CUDA_CHECK(cudaMemcpyAsync(hflags, d_gflags, sizeof(hflags), cudaMemcpyDeviceToHost, sh.stream));
+            HY_CUDA_CHECK(cudaStreamSynchronize(sh.stream));
         };
-        HY_CUDA_CHECK(cudaMemsetAsync(d_gflags, 0, sizeof(hflags), b->stream));
-        dev::k_grid_init<<<gb, 128, 0, b->stream>>>(b->view(), G, b->d_prop_min_h, b->d_prop_max_h, b->d_prop_n_steps);
-        dev::k_grid_sample<<<dim3(gb, b->n_eq), 128, 0, b->stream>>>(b->prog, b->view(), G);
-        dev::k_grid_advance<<<gb, 128, 0, b->stream>>>(b->view(), G);
+        HY_CUDA_CHECK(cudaMemsetAsync(d_gflags, 0, sizeof(hflags), sh.stream));
+        dev::k_grid_init<<<gb, 128, 0, sh.stream>>>(sh.view(), G, sh.d_prop_min_h, sh.d_prop_max_h, sh.d_prop_n_steps);
+        dev::k_grid_sample<<<dim3(gb, sh.n_eq), 128, 0, sh.stream>>>(sh.prog, sh.view(), G);
+        dev::k_grid_advance<<<gb, 128, 0, sh.stream>>>(sh.view(), G);
         HY_CUDA_CHECK(cudaGetLastError());
         read_flags();
         if (hflags[2] != 0u) {
@@ -2478,21 +2324,21 @@ int hy_batch_propagate_grid(hy_batch *b, const double *grid, uint64_t n_pts, con
             R.max_delta_t = G.dt_limit;
             R.default_max_delta_t = std::numeric_limits<double>::infinity();
             R.write_tc = 1;
-            R.flags = b->d_flags;
-            R.counter = b->d_counter;
-            b->launch(false, R);
-            HY_CUDA_CHECK(cudaMemsetAsync(d_gflags, 0, sizeof(unsigned) * 2u, b->stream));
-            dev::k_grid_book<<<gb, 128, 0, b->stream>>>(b->view(), G, b->d_prop_outcome, b->d_prop_min_h,
-                                                         b->d_prop_max_h, b->d_prop_n_steps);
-            dev::k_grid_sample<<<dim3(gb, b->n_eq), 128, 0, b->stream>>>(b->prog, b->view(), G);
-            dev::k_grid_advance<<<gb, 128, 0, b->stream>>>(b->view(), G);
+            R.flags = sh.d_flags;
+            R.counter = sh.d_counter;
+            sh.launch(false, R);
+            HY_CUDA_CHECK(cudaMemsetAsync(d_gflags, 0, sizeof(unsigned) * 2u, sh.stream));
+            dev::k_grid_book<<<gb, 128, 0, sh.stream>>>(sh.view(), G, sh.d_prop_outcome, sh.d_prop_min_h,
+                                                         sh.d_prop_max_h, sh.d_prop_n_steps);
+            dev::k_grid_sample<<<dim3(gb, sh.n_eq), 128, 0, sh.stream>>>(sh.prog, sh.view(), G);
+            dev::k_grid_advance<<<gb, 128, 0, sh.stream>>>(sh.view(), G);
             HY_CUDA_CHECK(cudaGetLastError());
             read_flags();
             if (hflags[1] != 0u) {
                 break; // non-finite state: nothing further is written (:1973-1978)
             }
             if (++iter == max_steps) {
-                dev::k_fill_outcome<<<(n + 255u) / 256u, 256, 0, b->stream>>>(b->d_prop_outcome, n,
+                dev::k_fill_outcome<<<(n + 255u) / 256u, 256, 0, sh.stream>>>(sh.d_prop_outcome, n,
                                                                               HY_OUTCOME_STEP_LIMIT);
                 interrupted = true;
             }
@@ -2557,9 +2403,10 @@ int hy_batch_propagate_until_cout_cb(hy_batch *b, const double *t_final_hi, cons
     unsigned char *d_dir = nullptr;
     unsigned *d_pflags = nullptr;
     bool tc_swapped = false;
+    shard *sh = nullptr;
     const auto cleanup = [&]() {
         if (tc_swapped) {
-            b->d_tc = own_tc;
+            sh->d_tc = own_tc;
         }
         for (void *ptr : {static_cast<void *>(d_lane), static_cast<void *>(d_dir), static_cast<void *>(d_pflags),
                           static_cast<void *>(d_times)}) {
@@ -2569,19 +2416,17 @@ int hy_batch_propagate_until_cout_cb(hy_batch *b, const double *t_final_hi, cons
         }
     };
     try {
-        if (b != nullptr && b->n_ev != 0u) {
-            throw hy::detail::not_implemented_error("A batch with event equations is propagated by the front end's lock-step "
-                                                    "loop over hy_batch_step(), not by the device-resident propagation");
-        }
-        if (b != nullptr && !b->shards.empty()) {
+        refuse_events(b);
+        if (b != nullptr && b->multi) {
             throw hy::detail::not_implemented_error("Continuous output is not available on a multi-device batch");
         }
         if (b == nullptr || t_final_hi == nullptr || out == nullptr) {
             throw std::invalid_argument("Null pointer passed to hy_batch_propagate_until_cout()");
         }
         *out = nullptr;
-        device_guard guard(b->device);
-        const std::uint32_t n = b->n;
+        sh = b->shards[0].get();
+        device_guard guard(sh->device);
+        const std::uint32_t n = sh->n;
         // Argument checks of propagate_until_impl(), src/taylor_adaptive_batch.cpp:1212-1241.
         for (std::uint32_t i = 0; i < n; ++i) {
             if (!std::isfinite(t_final_hi[i]) || (t_final_lo != nullptr && !std::isfinite(t_final_lo[i]))) {
@@ -2603,14 +2448,14 @@ int hy_batch_propagate_until_cout_cb(hy_batch *b, const double *t_final_hi, cons
         HY_CUDA_CHECK(cudaMalloc(&d_lane, sizeof(double) * 6u * n));
         HY_CUDA_CHECK(cudaMalloc(&d_dir, n));
         HY_CUDA_CHECK(cudaMalloc(&d_pflags, sizeof(unsigned) * 4u));
-        HY_CUDA_CHECK(cudaMemcpyAsync(d_lane + 4u * n, t_final_hi, sizeof(double) * n, cudaMemcpyHostToDevice, b->stream));
+        HY_CUDA_CHECK(cudaMemcpyAsync(d_lane + 4u * n, t_final_hi, sizeof(double) * n, cudaMemcpyHostToDevice, sh->stream));
         if (t_final_lo != nullptr) {
             HY_CUDA_CHECK(cudaMemcpyAsync(d_lane + 5u * n, t_final_lo, sizeof(double) * n, cudaMemcpyHostToDevice,
-                                          b->stream));
+                                          sh->stream));
         }
         if (max_delta_t != nullptr) {
             HY_CUDA_CHECK(cudaMemcpyAsync(d_lane + 3u * n, max_delta_t, sizeof(double) * n, cudaMemcpyHostToDevice,
-                                          b->stream));
+                                          sh->stream));
         }
         dev::prop_state G{};
         G.tf_hi = d_lane + 4u * n;
@@ -2622,19 +2467,19 @@ int hy_batch_propagate_until_cout_cb(hy_batch *b, const double *t_final_hi, cons
         G.dt_limit = d_lane + 2u * n;
         G.flags = d_pflags;
         const unsigned gb = (n + 127u) / 128u;
-        const std::size_t tc_doubles = static_cast<std::size_t>(b->n_eq) * (b->order + 1u) * n;
+        const std::size_t tc_doubles = static_cast<std::size_t>(sh->n_eq) * (sh->order + 1u) * n;
         unsigned hflags[4] = {0u, 0u, 0u, 0u};
         const auto read_flags = [&]() {
-            HY_CUDA_CHECK(cudaMemcpyAsync(hflags, d_pflags, sizeof(hflags), cudaMemcpyDeviceToHost, b->stream));
-            HY_CUDA_CHECK(cudaStreamSynchronize(b->stream));
+            HY_CUDA_CHECK(cudaMemcpyAsync(hflags, d_pflags, sizeof(hflags), cudaMemcpyDeviceToHost, sh->stream));
+            HY_CUDA_CHECK(cudaStreamSynchronize(sh->stream));
         };
         co = std::make_unique<hy_cout>();
-        co->device = b->device;
+        co->device = sh->device;
         co->n = n;
-        co->n_eq = b->n_eq;
-        co->order = b->order;
-        co->prog = b->prog;
-        co->stream = b->stream;
+        co->n_eq = sh->n_eq;
+        co->order = sh->order;
+        co->prog = sh->prog;
+        co->stream = sh->stream;
         // Slabs of about 64 MB (at least one iteration each).
         co->slab_iters = static_cast<std::uint32_t>(
             std::min<std::size_t>(std::max<std::size_t>((std::size_t(64) << 20) / (tc_doubles * sizeof(double)), 1u), 4096u));
@@ -2646,24 +2491,24 @@ int hy_batch_propagate_until_cout_cb(hy_batch *b, const double *t_final_hi, cons
                 HY_CUDA_CHECK(cudaMalloc(&nt, sizeof(double) * 2u * n * new_cap));
                 if (d_times != nullptr) {
                     HY_CUDA_CHECK(cudaMemcpyAsync(nt, d_times, sizeof(double) * 2u * n * times_rows, cudaMemcpyDeviceToDevice,
-                                                  b->stream));
-                    HY_CUDA_CHECK(cudaStreamSynchronize(b->stream));
+                                                  sh->stream));
+                    HY_CUDA_CHECK(cudaStreamSynchronize(sh->stream));
                     HY_CUDA_CHECK(cudaFree(d_times));
                 }
                 d_times = nt;
                 times_cap = new_cap;
             }
             double *blk = d_times + 2u * n * times_rows;
-            HY_CUDA_CHECK(cudaMemcpyAsync(blk, b->d_t_hi, sizeof(double) * n, cudaMemcpyDeviceToDevice, b->stream));
-            HY_CUDA_CHECK(cudaMemcpyAsync(blk + n, b->d_t_lo, sizeof(double) * n, cudaMemcpyDeviceToDevice, b->stream));
+            HY_CUDA_CHECK(cudaMemcpyAsync(blk, sh->d_t_hi, sizeof(double) * n, cudaMemcpyDeviceToDevice, sh->stream));
+            HY_CUDA_CHECK(cudaMemcpyAsync(blk + n, sh->d_t_lo, sizeof(double) * n, cudaMemcpyDeviceToDevice, sh->stream));
             ++times_rows;
         };
         push_times();
-        b->ensure_tc();
-        own_tc = b->d_tc;
+        sh->ensure_tc();
+        own_tc = sh->d_tc;
         tc_swapped = true;
-        HY_CUDA_CHECK(cudaMemsetAsync(d_pflags, 0, sizeof(hflags), b->stream));
-        dev::k_prop_init<<<gb, 128, 0, b->stream>>>(b->view(), G, b->d_prop_min_h, b->d_prop_max_h, b->d_prop_n_steps);
+        HY_CUDA_CHECK(cudaMemsetAsync(d_pflags, 0, sizeof(hflags), sh->stream));
+        dev::k_prop_init<<<gb, 128, 0, sh->stream>>>(sh->view(), G, sh->d_prop_min_h, sh->d_prop_max_h, sh->d_prop_n_steps);
         HY_CUDA_CHECK(cudaGetLastError());
         read_flags();
         if (hflags[2] != 0u) {
@@ -2678,17 +2523,17 @@ int hy_batch_propagate_until_cout_cb(hy_batch *b, const double *t_final_hi, cons
                 HY_CUDA_CHECK(cudaMalloc(&slab, sizeof(double) * tc_doubles * co->slab_iters));
                 co->slabs.push_back(slab);
             }
-            b->d_tc = co->slabs[iter / co->slab_iters] + (iter % co->slab_iters) * tc_doubles;
+            sh->d_tc = co->slabs[iter / co->slab_iters] + (iter % co->slab_iters) * tc_doubles;
             dev::run_args R{};
             R.max_delta_t = G.dt_limit;
             R.default_max_delta_t = std::numeric_limits<double>::infinity();
             R.write_tc = 1;
-            R.flags = b->d_flags;
-            R.counter = b->d_counter;
-            b->launch(false, R);
-            HY_CUDA_CHECK(cudaMemsetAsync(d_pflags, 0, sizeof(unsigned) * 2u, b->stream));
-            dev::k_prop_book<<<gb, 128, 0, b->stream>>>(b->view(), G, b->d_prop_outcome, b->d_prop_min_h,
-                                                         b->d_prop_max_h, b->d_prop_n_steps);
+            R.flags = sh->d_flags;
+            R.counter = sh->d_counter;
+            sh->launch(false, R);
+            HY_CUDA_CHECK(cudaMemsetAsync(d_pflags, 0, sizeof(unsigned) * 2u, sh->stream));
+            dev::k_prop_book<<<gb, 128, 0, sh->stream>>>(sh->view(), G, sh->d_prop_outcome, sh->d_prop_min_h,
+                                                         sh->d_prop_max_h, sh->d_prop_n_steps);
             HY_CUDA_CHECK(cudaGetLastError());
             read_flags();
             if (hflags[1] != 0u) {
@@ -2699,13 +2544,13 @@ int hy_batch_propagate_until_cout_cb(hy_batch *b, const double *t_final_hi, cons
             ++iter;
             if (cb != nullptr) {
                 // The step callback (:1476-1500), before the exit tests like in the reference.
-                HY_CUDA_CHECK(cudaStreamSynchronize(b->stream));
+                HY_CUDA_CHECK(cudaStreamSynchronize(sh->stream));
                 const int r = cb(user);
                 if (r < 0) {
                     throw callback_abort{};
                 }
                 if (r == 0) {
-                    dev::k_fill_outcome<<<(n + 255u) / 256u, 256, 0, b->stream>>>(b->d_prop_outcome, n,
+                    dev::k_fill_outcome<<<(n + 255u) / 256u, 256, 0, sh->stream>>>(sh->d_prop_outcome, n,
                                                                                   HY_OUTCOME_CB_STOP);
                     break;
                 }
@@ -2714,14 +2559,14 @@ int hy_batch_propagate_until_cout_cb(hy_batch *b, const double *t_final_hi, cons
                 break; // every lane reached its final time
             }
             if (iter == max_steps) {
-                dev::k_fill_outcome<<<(n + 255u) / 256u, 256, 0, b->stream>>>(b->d_prop_outcome, n,
+                dev::k_fill_outcome<<<(n + 255u) / 256u, 256, 0, sh->stream>>>(sh->d_prop_outcome, n,
                                                                               HY_OUTCOME_STEP_LIMIT);
                 break;
             }
         }
         // The batch's own tc array ends up with the coefficients of the last step taken, like m_tc in the reference.
-        HY_CUDA_CHECK(cudaMemcpyAsync(own_tc, b->d_tc, sizeof(double) * tc_doubles, cudaMemcpyDeviceToDevice, b->stream));
-        b->d_tc = own_tc;
+        HY_CUDA_CHECK(cudaMemcpyAsync(own_tc, sh->d_tc, sizeof(double) * tc_doubles, cudaMemcpyDeviceToDevice, sh->stream));
+        sh->d_tc = own_tc;
         tc_swapped = false;
         if (iter != 0u) {
             // make_c_out(), :1277-1317: the times get a padding row, +-inf by direction.
@@ -2730,17 +2575,17 @@ int hy_batch_propagate_until_cout_cb(hy_batch *b, const double *t_final_hi, cons
             HY_CUDA_CHECK(cudaMalloc(&co->d_t_hi, sizeof(double) * rows * n));
             HY_CUDA_CHECK(cudaMalloc(&co->d_t_lo, sizeof(double) * rows * n));
             HY_CUDA_CHECK(cudaMalloc(&co->d_tm, sizeof(double) * n));
-            HY_CUDA_CHECK(cudaMalloc(&co->d_out, sizeof(double) * static_cast<std::size_t>(b->n_eq) * n));
+            HY_CUDA_CHECK(cudaMalloc(&co->d_out, sizeof(double) * static_cast<std::size_t>(sh->n_eq) * n));
             HY_CUDA_CHECK(cudaMemcpy2DAsync(co->d_t_hi, sizeof(double) * n, d_times, sizeof(double) * 2u * n,
-                                            sizeof(double) * n, iter + 1u, cudaMemcpyDeviceToDevice, b->stream));
+                                            sizeof(double) * n, iter + 1u, cudaMemcpyDeviceToDevice, sh->stream));
             HY_CUDA_CHECK(cudaMemcpy2DAsync(co->d_t_lo, sizeof(double) * n, d_times + n, sizeof(double) * 2u * n,
-                                            sizeof(double) * n, iter + 1u, cudaMemcpyDeviceToDevice, b->stream));
+                                            sizeof(double) * n, iter + 1u, cudaMemcpyDeviceToDevice, sh->stream));
             HY_CUDA_CHECK(cudaMalloc(&co->d_slabs, sizeof(double *) * co->slabs.size()));
             HY_CUDA_CHECK(cudaMemcpyAsync(co->d_slabs, co->slabs.data(), sizeof(double *) * co->slabs.size(),
-                                          cudaMemcpyHostToDevice, b->stream));
+                                          cudaMemcpyHostToDevice, sh->stream));
             std::vector<unsigned char> dir(n);
-            HY_CUDA_CHECK(cudaMemcpyAsync(dir.data(), d_dir, n, cudaMemcpyDeviceToHost, b->stream));
-            HY_CUDA_CHECK(cudaStreamSynchronize(b->stream));
+            HY_CUDA_CHECK(cudaMemcpyAsync(dir.data(), d_dir, n, cudaMemcpyDeviceToHost, sh->stream));
+            HY_CUDA_CHECK(cudaStreamSynchronize(sh->stream));
             std::vector<double> pad(n), zero(n, 0.);
             for (std::uint32_t i = 0; i < n; ++i) {
                 pad[i] = dir[i] != 0 ? std::numeric_limits<double>::infinity() : -std::numeric_limits<double>::infinity();
@@ -2749,7 +2594,7 @@ int hy_batch_propagate_until_cout_cb(hy_batch *b, const double *t_final_hi, cons
             HY_CUDA_CHECK(cudaMemcpy(co->d_t_lo + (rows - 1u) * n, zero.data(), sizeof(double) * n, cudaMemcpyHostToDevice));
             *out = co.release();
         }
-        HY_CUDA_CHECK(cudaStreamSynchronize(b->stream));
+        HY_CUDA_CHECK(cudaStreamSynchronize(sh->stream));
         cleanup();
         return HY_OK;
     } catch (const callback_abort &) {
@@ -2781,25 +2626,25 @@ struct hy_cout_rec {
 namespace
 {
 
-void rec_push_times(hy_batch *b, hy_cout_rec *r)
+void rec_push_times(shard &sh, hy_cout_rec *r)
 {
-    const std::uint32_t n = b->n;
+    const std::uint32_t n = sh.n;
     if (r->times_rows == r->times_cap) {
         const std::size_t new_cap = std::max<std::size_t>(2u * r->times_cap, 64u);
         double *nt = nullptr;
         HY_CUDA_CHECK(cudaMalloc(&nt, sizeof(double) * 2u * n * new_cap));
         if (r->d_times != nullptr) {
             HY_CUDA_CHECK(cudaMemcpyAsync(nt, r->d_times, sizeof(double) * 2u * n * r->times_rows, cudaMemcpyDeviceToDevice,
-                                          b->stream));
-            HY_CUDA_CHECK(cudaStreamSynchronize(b->stream));
+                                          sh.stream));
+            HY_CUDA_CHECK(cudaStreamSynchronize(sh.stream));
             HY_CUDA_CHECK(cudaFree(r->d_times));
         }
         r->d_times = nt;
         r->times_cap = new_cap;
     }
     double *blk = r->d_times + 2u * n * r->times_rows;
-    HY_CUDA_CHECK(cudaMemcpyAsync(blk, b->d_t_hi, sizeof(double) * n, cudaMemcpyDeviceToDevice, b->stream));
-    HY_CUDA_CHECK(cudaMemcpyAsync(blk + n, b->d_t_lo, sizeof(double) * n, cudaMemcpyDeviceToDevice, b->stream));
+    HY_CUDA_CHECK(cudaMemcpyAsync(blk, sh.d_t_hi, sizeof(double) * n, cudaMemcpyDeviceToDevice, sh.stream));
+    HY_CUDA_CHECK(cudaMemcpyAsync(blk + n, sh.d_t_lo, sizeof(double) * n, cudaMemcpyDeviceToDevice, sh.stream));
     ++r->times_rows;
 }
 
@@ -2811,24 +2656,25 @@ int hy_cout_rec_begin(hy_batch *b, hy_cout_rec **out)
         if (b == nullptr || out == nullptr) {
             throw std::invalid_argument("Null pointer passed to hy_cout_rec_begin()");
         }
-        if (!b->shards.empty()) {
+        if (b->multi) {
             throw hy::detail::not_implemented_error("Continuous output is not available on a multi-device batch");
         }
         *out = nullptr;
-        device_guard guard(b->device);
+        shard &sh = *b->shards[0];
+        device_guard guard(sh.device);
         auto r = std::make_unique<hy_cout_rec>();
-        r->tc_doubles = static_cast<std::size_t>(b->n_eq) * (b->order + 1u) * b->n;
+        r->tc_doubles = static_cast<std::size_t>(sh.n_eq) * (sh.order + 1u) * sh.n;
         r->co = std::make_unique<hy_cout>();
-        r->co->device = b->device;
-        r->co->n = b->n;
-        r->co->n_eq = b->n_eq;
-        r->co->order = b->order;
-        r->co->prog = b->prog;
-        r->co->stream = b->stream;
+        r->co->device = sh.device;
+        r->co->n = sh.n;
+        r->co->n_eq = sh.n_eq;
+        r->co->order = sh.order;
+        r->co->prog = sh.prog;
+        r->co->stream = sh.stream;
         r->co->slab_iters = static_cast<std::uint32_t>(std::min<std::size_t>(
             std::max<std::size_t>((std::size_t(64) << 20) / (r->tc_doubles * sizeof(double)), 1u), 4096u));
-        rec_push_times(b, r.get()); // row 0: the starting time
-        HY_CUDA_CHECK(cudaStreamSynchronize(b->stream));
+        rec_push_times(sh, r.get()); // row 0: the starting time
+        HY_CUDA_CHECK(cudaStreamSynchronize(sh.stream));
         *out = r.release();
         return HY_OK;
     } catch (...) {
@@ -2839,11 +2685,13 @@ int hy_cout_rec_begin(hy_batch *b, hy_cout_rec **out)
 int hy_cout_rec_append(hy_batch *b, hy_cout_rec *r)
 {
     try {
-        if (b == nullptr || r == nullptr || r->co == nullptr || r->co->n != b->n || b->d_tc == nullptr) {
+        if (b == nullptr || b->multi || r == nullptr || r->co == nullptr || r->co->n != b->n
+            || b->shards[0]->d_tc == nullptr) {
             throw std::invalid_argument("Invalid arguments passed to hy_cout_rec_append() (the last step must have "
                                         "written its Taylor coefficients)");
         }
-        device_guard guard(b->device);
+        shard &sh = *b->shards[0];
+        device_guard guard(sh.device);
         auto &co = *r->co;
         if (r->iter / co.slab_iters == co.slabs.size()) {
             double *slab = nullptr;
@@ -2851,9 +2699,9 @@ int hy_cout_rec_append(hy_batch *b, hy_cout_rec *r)
             co.slabs.push_back(slab);
         }
         // (The rows of the state variables come first in the batch's tc array; those of event equations are not recorded.)
-        HY_CUDA_CHECK(cudaMemcpyAsync(co.slabs[r->iter / co.slab_iters] + (r->iter % co.slab_iters) * r->tc_doubles, b->d_tc,
-                                      sizeof(double) * r->tc_doubles, cudaMemcpyDeviceToDevice, b->stream));
-        rec_push_times(b, r);
+        HY_CUDA_CHECK(cudaMemcpyAsync(co.slabs[r->iter / co.slab_iters] + (r->iter % co.slab_iters) * r->tc_doubles, sh.d_tc,
+                                      sizeof(double) * r->tc_doubles, cudaMemcpyDeviceToDevice, sh.stream));
+        rec_push_times(sh, r);
         ++r->iter;
         return HY_OK;
     } catch (...) {
@@ -2876,8 +2724,9 @@ int hy_cout_rec_finish(hy_batch *b, hy_cout_rec *rp, const unsigned char *forwar
             throw std::invalid_argument("Null pointer passed to hy_cout_rec_finish()");
         }
         *out = nullptr;
-        device_guard guard(b->device);
-        const std::uint32_t n = b->n;
+        shard &sh = *b->shards[0];
+        device_guard guard(sh.device);
+        const std::uint32_t n = sh.n;
         const std::uint64_t iter = r->iter;
         if (iter != 0u) {
             auto &co = *r->co;
@@ -2886,15 +2735,15 @@ int hy_cout_rec_finish(hy_batch *b, hy_cout_rec *rp, const unsigned char *forwar
             HY_CUDA_CHECK(cudaMalloc(&co.d_t_hi, sizeof(double) * rows * n));
             HY_CUDA_CHECK(cudaMalloc(&co.d_t_lo, sizeof(double) * rows * n));
             HY_CUDA_CHECK(cudaMalloc(&co.d_tm, sizeof(double) * n));
-            HY_CUDA_CHECK(cudaMalloc(&co.d_out, sizeof(double) * static_cast<std::size_t>(b->n_eq) * n));
+            HY_CUDA_CHECK(cudaMalloc(&co.d_out, sizeof(double) * static_cast<std::size_t>(sh.n_eq) * n));
             HY_CUDA_CHECK(cudaMemcpy2DAsync(co.d_t_hi, sizeof(double) * n, r->d_times, sizeof(double) * 2u * n,
-                                            sizeof(double) * n, iter + 1u, cudaMemcpyDeviceToDevice, b->stream));
+                                            sizeof(double) * n, iter + 1u, cudaMemcpyDeviceToDevice, sh.stream));
             HY_CUDA_CHECK(cudaMemcpy2DAsync(co.d_t_lo, sizeof(double) * n, r->d_times + n, sizeof(double) * 2u * n,
-                                            sizeof(double) * n, iter + 1u, cudaMemcpyDeviceToDevice, b->stream));
+                                            sizeof(double) * n, iter + 1u, cudaMemcpyDeviceToDevice, sh.stream));
             HY_CUDA_CHECK(cudaMalloc(&co.d_slabs, sizeof(double *) * co.slabs.size()));
             HY_CUDA_CHECK(cudaMemcpyAsync(co.d_slabs, co.slabs.data(), sizeof(double *) * co.slabs.size(),
-                                          cudaMemcpyHostToDevice, b->stream));
-            HY_CUDA_CHECK(cudaStreamSynchronize(b->stream));
+                                          cudaMemcpyHostToDevice, sh.stream));
+            HY_CUDA_CHECK(cudaStreamSynchronize(sh.stream));
             std::vector<double> pad(n), zero(n, 0.);
             for (std::uint32_t i = 0; i < n; ++i) {
                 pad[i] = forward[i] != 0 ? std::numeric_limits<double>::infinity() : -std::numeric_limits<double>::infinity();
@@ -2903,7 +2752,7 @@ int hy_cout_rec_finish(hy_batch *b, hy_cout_rec *rp, const unsigned char *forwar
             HY_CUDA_CHECK(cudaMemcpy(co.d_t_lo + (rows - 1u) * n, zero.data(), sizeof(double) * n, cudaMemcpyHostToDevice));
             *out = r->co.release();
         }
-        HY_CUDA_CHECK(cudaStreamSynchronize(b->stream));
+        HY_CUDA_CHECK(cudaStreamSynchronize(sh.stream));
         return HY_OK;
     } catch (...) {
         return translate_exception();
@@ -3000,30 +2849,18 @@ void hy_cout_destroy(hy_cout *c)
 int hy_batch_d_output(hy_batch *b, const double *tau, double *out)
 {
     try {
-        if (!b->shards.empty()) {
-            for_each_shard(b, [&](hy_batch *sh, std::size_t i) {
-                const double *d_tau = stage(sh, tau + b->shard_off[i], 0, 0);
-                sh->ensure_tc();
-                dev::k_d_output<<<(sh->n + 127u) / 128u, 128, 0, sh->stream>>>(sh->prog, sh->n, sh->d_tc, d_tau,
-                                                                              sh->d_d_out);
-                HY_CUDA_CHECK(cudaGetLastError());
-                ++sh->n_launches;
-                rows_d2h(sh, out, sh->d_d_out, sh->n_eq, b->n, b->shard_off[i]);
-                HY_CUDA_CHECK(cudaStreamSynchronize(sh->stream));
-            });
-            return HY_OK;
+        if (b == nullptr || tau == nullptr) {
+            throw std::invalid_argument("Null pointer passed to hy_batch_d_output()");
         }
-        device_guard guard(b->device);
-        const double *d_tau = stage(b, tau, 0, 0);
-        b->ensure_tc();
-        dev::k_d_output<<<(b->n + 127u) / 128u, 128, 0, b->stream>>>(b->prog, b->n, b->d_tc, d_tau, b->d_d_out);
-        HY_CUDA_CHECK(cudaGetLastError());
-        ++b->n_launches;
-        if (out != nullptr) {
-            HY_CUDA_CHECK(cudaMemcpyAsync(out, b->d_d_out, sizeof(double) * b->n * b->n_eq, cudaMemcpyDeviceToHost,
-                                          b->stream));
-        }
-        HY_CUDA_CHECK(cudaStreamSynchronize(b->stream));
+        for_each_shard(b, [&](shard &sh, std::size_t i) {
+            const double *d_tau = stage(sh, tau, 0, b->off[i], 0);
+            sh.ensure_tc();
+            dev::k_d_output<<<(sh.n + 127u) / 128u, 128, 0, sh.stream>>>(sh.prog, sh.n, sh.d_tc, d_tau, sh.d_d_out);
+            HY_CUDA_CHECK(cudaGetLastError());
+            ++sh.n_launches;
+            rows_d2h(sh, out, sh.d_d_out, sh.n_eq, b->n, b->off[i]);
+            HY_CUDA_CHECK(cudaStreamSynchronize(sh.stream));
+        });
         return HY_OK;
     } catch (...) {
         return translate_exception();
@@ -3033,37 +2870,37 @@ int hy_batch_d_output(hy_batch *b, const double *tau, double *out)
 namespace
 {
 
-// k_taylor_map on one single-device batch, device-resident dx / out.
-void taylor_map_launch(hy_batch *b, std::uint32_t n_orig, std::uint32_t m, const double *d_dx, double *d_out)
+// k_taylor_map on one shard, device-resident dx / out.
+void taylor_map_launch(shard &sh, std::uint32_t n_orig, std::uint32_t m, const double *d_dx, double *d_out)
 {
     const std::uint32_t chunk = std::min(m, dev::TMAP_CHUNK);
-    dev::k_taylor_map<<<(b->n + dev::TMAP_THREADS - 1u) / dev::TMAP_THREADS, dev::TMAP_THREADS,
-                        sizeof(double) * chunk * dev::TMAP_THREADS, b->stream>>>(b->d_state, b->n, n_orig, m, d_dx,
+    dev::k_taylor_map<<<(sh.n + dev::TMAP_THREADS - 1u) / dev::TMAP_THREADS, dev::TMAP_THREADS,
+                        sizeof(double) * chunk * dev::TMAP_THREADS, sh.stream>>>(sh.d_state, sh.n, n_orig, m, d_dx,
                                                                                  d_out);
     HY_CUDA_CHECK(cudaGetLastError());
-    ++b->n_launches;
+    ++sh.n_launches;
 }
 
 // Host form: dx staged into d_tmap[0, m * n), the result read back from d_tmap[m * n, (m + n_orig) * n).
-void taylor_map_host(hy_batch *b, std::uint32_t n_orig, std::uint32_t m, const double *dx, double *out,
+void taylor_map_host(shard &sh, std::uint32_t n_orig, std::uint32_t m, const double *dx, double *out,
                      std::size_t pitch, std::size_t off)
 {
-    const std::size_t need = static_cast<std::size_t>(m + n_orig) * b->n;
-    if (b->tmap_doubles < need) {
-        if (b->d_tmap != nullptr) {
-            HY_CUDA_CHECK(cudaStreamSynchronize(b->stream));
-            HY_CUDA_CHECK(cudaFree(b->d_tmap));
-            b->d_tmap = nullptr;
-            b->tmap_doubles = 0;
+    const std::size_t need = static_cast<std::size_t>(m + n_orig) * sh.n;
+    if (sh.tmap_doubles < need) {
+        if (sh.d_tmap != nullptr) {
+            HY_CUDA_CHECK(cudaStreamSynchronize(sh.stream));
+            HY_CUDA_CHECK(cudaFree(sh.d_tmap));
+            sh.d_tmap = nullptr;
+            sh.tmap_doubles = 0;
         }
-        b->d_tmap = b->dalloc<double>(need);
-        b->tmap_doubles = need;
+        sh.d_tmap = sh.dalloc<double>(need);
+        sh.tmap_doubles = need;
     }
-    double *d_dx = b->d_tmap, *d_out = b->d_tmap + static_cast<std::size_t>(m) * b->n;
-    rows_h2d(b, d_dx, dx, m, pitch, off);
-    taylor_map_launch(b, n_orig, m, d_dx, d_out);
-    rows_d2h(b, out, d_out, n_orig, pitch, off);
-    HY_CUDA_CHECK(cudaStreamSynchronize(b->stream));
+    double *d_dx = sh.d_tmap, *d_out = sh.d_tmap + static_cast<std::size_t>(m) * sh.n;
+    rows_h2d(sh, d_dx, dx, m, pitch, off);
+    taylor_map_launch(sh, n_orig, m, d_dx, d_out);
+    rows_d2h(sh, out, d_out, n_orig, pitch, off);
+    HY_CUDA_CHECK(cudaStreamSynchronize(sh.stream));
 }
 
 } // namespace
@@ -3083,24 +2920,18 @@ int hy_batch_eval_taylor_map(hy_batch *b, uint32_t n_orig_sv, uint32_t n_args, c
                 + " arguments do not make a variational system of order 1 with " + std::to_string(b->n_eq)
                 + " equations");
         }
-        if (!b->shards.empty()) {
+        if (on_device && b->multi) {
+            throw std::invalid_argument(
+                "Device-resident arrays are not available for the Taylor map of a multi-device batch");
+        }
+        for_each_shard(b, [&](shard &sh, std::size_t i) {
             if (on_device) {
-                throw std::invalid_argument(
-                    "Device-resident arrays are not available for the Taylor map of a multi-device batch");
+                // (Asynchronous on the batch's stream, like the other device-resident entry points.)
+                taylor_map_launch(sh, n_orig_sv, n_args, dx, out);
+            } else {
+                taylor_map_host(sh, n_orig_sv, n_args, dx, out, b->n, b->off[i]);
             }
-            // Every shard evaluates its own lanes on its own device.
-            for_each_shard(b, [&](hy_batch *sh, std::size_t i) {
-                taylor_map_host(sh, n_orig_sv, n_args, dx, out, b->n, b->shard_off[i]);
-            });
-            return HY_OK;
-        }
-        device_guard guard(b->device);
-        if (on_device) {
-            // (Asynchronous on the batch's stream, like the other device-resident entry points.)
-            taylor_map_launch(b, n_orig_sv, n_args, dx, out);
-        } else {
-            taylor_map_host(b, n_orig_sv, n_args, dx, out, b->n, 0);
-        }
+        });
         return HY_OK;
     } catch (...) {
         return translate_exception();
@@ -3114,21 +2945,30 @@ int hy_batch_set_events(hy_batch *b, uint32_t n_te, const int32_t *dirs, const d
         if (b == nullptr || dirs == nullptr || (n_te != 0u && cooldowns == nullptr)) {
             throw std::invalid_argument("Null pointer passed to hy_batch_set_events()");
         }
-        if (!b->shards.empty()) {
-            // (Directions, cooldowns and tolerance are per event, not per lane: every shard gets them all.)
-            for (auto *sh : b->shards) {
-                if (hy_batch_set_events(sh, n_te, dirs, cooldowns, tol) != HY_OK) {
-                    throw std::invalid_argument(hy_last_error());
-                }
-            }
-            b->n_te = n_te;
-            b->ev_set = true;
-            b->ev_host.clear();
-            return HY_OK;
+        if (b->n_ev == 0u) {
+            throw std::invalid_argument("This batch was built from a program without event equations");
         }
-        device_guard guard(b->device);
-        HY_CUDA_CHECK(cudaStreamSynchronize(b->stream));
-        b->ev_setup(n_te, dirs, cooldowns, tol);
+        if (n_te > b->n_ev) {
+            throw std::invalid_argument("The number of terminal events exceeds the number of event equations");
+        }
+        for (std::uint32_t k = 0; k < b->n_ev; ++k) {
+            if (dirs[k] < -1 || dirs[k] > 1) {
+                throw std::invalid_argument("Invalid value selected for the direction of an event");
+            }
+        }
+        for (std::uint32_t k = 0; k < n_te; ++k) {
+            if (!std::isfinite(cooldowns[k])) {
+                throw std::invalid_argument("Cannot set a non-finite cooldown value for a terminal event");
+            }
+        }
+        // (Directions, cooldowns and tolerance are per event, not per lane: every shard gets them all.)
+        for_each_shard(b, [&](shard &sh, std::size_t) {
+            HY_CUDA_CHECK(cudaStreamSynchronize(sh.stream));
+            sh.ev_setup(n_te, dirs, cooldowns, tol);
+        });
+        b->n_te = n_te;
+        b->ev_set = true;
+        b->ev_host.clear();
         return HY_OK;
     } catch (...) {
         return translate_exception();
@@ -3157,26 +2997,16 @@ int hy_batch_download_tc_events(hy_batch *b, double *out)
         if (b == nullptr || out == nullptr) {
             throw std::invalid_argument("Null pointer passed to hy_batch_download_tc_events()");
         }
-        if (!b->shards.empty()) {
-            for_each_shard(b, [&](hy_batch *sh, std::size_t i) {
-                if (sh->n_ev == 0u || sh->d_tc == nullptr) {
-                    throw std::invalid_argument("No Taylor coefficients of event equations are available");
-                }
-                const std::size_t rows = static_cast<std::size_t>(sh->order + 1u) * sh->n_ev;
-                rows_d2h(sh, out, sh->d_tc + static_cast<std::size_t>(sh->order + 1u) * sh->n * sh->n_eq, rows, b->n,
-                         b->shard_off[i]);
-                HY_CUDA_CHECK(cudaStreamSynchronize(sh->stream));
-            });
-            return HY_OK;
-        }
-        if (b->n_ev == 0u || b->d_tc == nullptr) {
+        if (b->n_ev == 0u
+            || std::any_of(b->shards.begin(), b->shards.end(), [](const auto &sh) { return sh->d_tc == nullptr; })) {
             throw std::invalid_argument("No Taylor coefficients of event equations are available");
         }
-        device_guard guard(b->device);
-        const std::size_t row = static_cast<std::size_t>(b->order + 1u) * b->n;
-        HY_CUDA_CHECK(cudaMemcpyAsync(out, b->d_tc + row * b->n_eq, sizeof(double) * row * b->n_ev, cudaMemcpyDeviceToHost,
-                                      b->stream));
-        HY_CUDA_CHECK(cudaStreamSynchronize(b->stream));
+        for_each_shard(b, [&](shard &sh, std::size_t i) {
+            // (The rows of the event equations follow those of the state variables.)
+            const std::size_t rows = static_cast<std::size_t>(sh.order + 1u) * sh.n_ev;
+            rows_d2h(sh, out, sh.d_tc + static_cast<std::size_t>(sh.order + 1u) * sh.n * sh.n_eq, rows, b->n, b->off[i]);
+            HY_CUDA_CHECK(cudaStreamSynchronize(sh.stream));
+        });
         return HY_OK;
     } catch (...) {
         return translate_exception();
@@ -3196,72 +3026,42 @@ int hy_batch_reset_cooldowns(hy_batch *b, int64_t lane)
             throw std::invalid_argument("Cannot reset the cooldowns at batch index " + std::to_string(lane)
                                         + ": the batch size for this integrator is only " + std::to_string(b->n));
         }
-        if (!b->shards.empty()) {
-            for (std::size_t i = 0; i < b->shards.size(); ++i) {
-                const auto lo = static_cast<int64_t>(b->shard_off[i]), hi = static_cast<int64_t>(b->shard_off[i + 1u]);
-                if (lane < 0 || (lane >= lo && lane < hi)) {
-                    if (hy_batch_reset_cooldowns(b->shards[i], lane < 0 ? lane : lane - lo) != HY_OK) {
-                        throw std::invalid_argument(hy_last_error());
-                    }
-                }
+        for_each_shard(b, [&](shard &sh, std::size_t i) {
+            const auto lo = static_cast<int64_t>(b->off[i]);
+            const std::size_t m = static_cast<std::size_t>(b->n_te) * sh.n;
+            if (m == 0u || (lane >= 0 && (lane < lo || lane >= lo + sh.n))) {
+                return;
             }
-            return HY_OK;
-        }
-        device_guard guard(b->device);
-        const std::size_t m = static_cast<std::size_t>(b->n_te) * b->n;
-        if (m != 0u) {
-            dev::k_ev_reset_cd<<<static_cast<unsigned>((m + 255u) / 256u), 256, 0, b->stream>>>(
-                b->eva, b->n, lane < 0 ? 0xffffffffu : static_cast<std::uint32_t>(lane));
+            dev::k_ev_reset_cd<<<static_cast<unsigned>((m + 255u) / 256u), 256, 0, sh.stream>>>(
+                sh.eva, sh.n, lane < 0 ? 0xffffffffu : static_cast<std::uint32_t>(lane - lo));
             HY_CUDA_CHECK(cudaGetLastError());
-        }
+        });
         return HY_OK;
     } catch (...) {
         return translate_exception();
     }
 }
 
+// The cooldown state [n_te][batch] is gathered / scattered by columns: every shard keeps its lanes' active flags as
+// [n_te][lanes] and the time spent and the cooldown as [n_te][2][lanes].
 int hy_batch_get_cooldowns(hy_batch *b, uint8_t *active, double *spent, double *cooldown)
 {
     try {
         if (b == nullptr || !b->ev_set) {
             throw std::invalid_argument("No events are defined for this integrator");
         }
-        if (!b->shards.empty()) {
-            // [n_te][batch] arrays: every shard fills its columns.
-            for (std::size_t i = 0; i < b->shards.size(); ++i) {
-                hy_batch *sh = b->shards[i];
-                const std::size_t ms = static_cast<std::size_t>(b->n_te) * sh->n;
-                std::vector<uint8_t> a(ms);
-                std::vector<double> sp(ms), cdw(ms);
-                if (hy_batch_get_cooldowns(sh, a.data(), sp.data(), cdw.data()) != HY_OK) {
-                    throw std::invalid_argument(hy_last_error());
-                }
-                for (std::uint32_t k = 0; k < b->n_te; ++k) {
-                    for (std::uint32_t l = 0; l < sh->n; ++l) {
-                        const std::size_t dst = static_cast<std::size_t>(k) * b->n + b->shard_off[i] + l,
-                                          src = static_cast<std::size_t>(k) * sh->n + l;
-                        active[dst] = a[src];
-                        spent[dst] = sp[src];
-                        cooldown[dst] = cdw[src];
-                    }
-                }
+        if (b->n_te != 0u && (active == nullptr || spent == nullptr || cooldown == nullptr)) {
+            throw std::invalid_argument("Null pointer passed to hy_batch_get_cooldowns()");
+        }
+        for_each_shard(b, [&](shard &sh, std::size_t i) {
+            rows_d2h(sh, active, sh.eva.cd_on, b->n_te, b->n, b->off[i]);
+            for (std::uint32_t k = 0; k < b->n_te; ++k) {
+                const std::size_t row = static_cast<std::size_t>(k) * b->n;
+                rows_d2h(sh, spent + row, sh.eva.cd + static_cast<std::size_t>(2u * k) * sh.n, 1u, b->n, b->off[i]);
+                rows_d2h(sh, cooldown + row, sh.eva.cd + static_cast<std::size_t>(2u * k + 1u) * sh.n, 1u, b->n, b->off[i]);
             }
-            return HY_OK;
-        }
-        device_guard guard(b->device);
-        const std::size_t m = static_cast<std::size_t>(b->n_te) * b->n;
-        std::vector<double> cd(2u * m);
-        if (m != 0u) {
-            HY_CUDA_CHECK(cudaMemcpyAsync(active, b->eva.cd_on, m, cudaMemcpyDeviceToHost, b->stream));
-            HY_CUDA_CHECK(cudaMemcpyAsync(cd.data(), b->eva.cd, sizeof(double) * 2u * m, cudaMemcpyDeviceToHost, b->stream));
-        }
-        HY_CUDA_CHECK(cudaStreamSynchronize(b->stream));
-        for (std::uint32_t k = 0; k < b->n_te; ++k) {
-            for (std::uint32_t l = 0; l < b->n; ++l) {
-                spent[static_cast<std::size_t>(k) * b->n + l] = cd[(static_cast<std::size_t>(k) * 2u) * b->n + l];
-                cooldown[static_cast<std::size_t>(k) * b->n + l] = cd[(static_cast<std::size_t>(k) * 2u + 1u) * b->n + l];
-            }
-        }
+            HY_CUDA_CHECK(cudaStreamSynchronize(sh.stream));
+        });
         return HY_OK;
     } catch (...) {
         return translate_exception();
@@ -3274,47 +3074,18 @@ int hy_batch_set_cooldowns(hy_batch *b, const uint8_t *active, const double *spe
         if (b == nullptr || !b->ev_set) {
             throw std::invalid_argument("No events are defined for this integrator");
         }
-        if (!b->shards.empty()) {
-            if (b->n_te != 0u && (active == nullptr || spent == nullptr || cooldown == nullptr)) {
-                throw std::invalid_argument("Null pointer passed to hy_batch_set_cooldowns()");
-            }
-            for (std::size_t i = 0; i < b->shards.size(); ++i) {
-                hy_batch *sh = b->shards[i];
-                const std::size_t ms = static_cast<std::size_t>(b->n_te) * sh->n;
-                std::vector<uint8_t> a(ms);
-                std::vector<double> sp(ms), cdw(ms);
-                for (std::uint32_t k = 0; k < b->n_te; ++k) {
-                    for (std::uint32_t l = 0; l < sh->n; ++l) {
-                        const std::size_t src = static_cast<std::size_t>(k) * b->n + b->shard_off[i] + l,
-                                          dst = static_cast<std::size_t>(k) * sh->n + l;
-                        a[dst] = active[src];
-                        sp[dst] = spent[src];
-                        cdw[dst] = cooldown[src];
-                    }
-                }
-                if (hy_batch_set_cooldowns(sh, a.data(), sp.data(), cdw.data()) != HY_OK) {
-                    throw std::invalid_argument(hy_last_error());
-                }
-            }
-            return HY_OK;
+        if (b->n_te != 0u && (active == nullptr || spent == nullptr || cooldown == nullptr)) {
+            throw std::invalid_argument("Null pointer passed to hy_batch_set_cooldowns()");
         }
-        device_guard guard(b->device);
-        const std::size_t m = static_cast<std::size_t>(b->n_te) * b->n;
-        if (m != 0u) {
-            if (active == nullptr || spent == nullptr || cooldown == nullptr) {
-                throw std::invalid_argument("Null pointer passed to hy_batch_set_cooldowns()");
-            }
-            std::vector<double> cd(2u * m);
+        for_each_shard(b, [&](shard &sh, std::size_t i) {
+            rows_h2d(sh, sh.eva.cd_on, active, b->n_te, b->n, b->off[i]);
             for (std::uint32_t k = 0; k < b->n_te; ++k) {
-                for (std::uint32_t l = 0; l < b->n; ++l) {
-                    cd[(static_cast<std::size_t>(k) * 2u) * b->n + l] = spent[static_cast<std::size_t>(k) * b->n + l];
-                    cd[(static_cast<std::size_t>(k) * 2u + 1u) * b->n + l] = cooldown[static_cast<std::size_t>(k) * b->n + l];
-                }
+                const std::size_t row = static_cast<std::size_t>(k) * b->n;
+                rows_h2d(sh, sh.eva.cd + static_cast<std::size_t>(2u * k) * sh.n, spent + row, 1u, b->n, b->off[i]);
+                rows_h2d(sh, sh.eva.cd + static_cast<std::size_t>(2u * k + 1u) * sh.n, cooldown + row, 1u, b->n, b->off[i]);
             }
-            HY_CUDA_CHECK(cudaMemcpyAsync(b->eva.cd_on, active, m, cudaMemcpyHostToDevice, b->stream));
-            HY_CUDA_CHECK(cudaMemcpyAsync(b->eva.cd, cd.data(), sizeof(double) * 2u * m, cudaMemcpyHostToDevice, b->stream));
-            HY_CUDA_CHECK(cudaStreamSynchronize(b->stream));
-        }
+            HY_CUDA_CHECK(cudaStreamSynchronize(sh.stream));
+        });
         return HY_OK;
     } catch (...) {
         return translate_exception();
@@ -3327,8 +3098,8 @@ int hy_batch_launch_count(const hy_batch *b, uint64_t *n_launches)
         hy::detail::set_last_error("Null pointer passed to hy_batch_launch_count()");
         return HY_ERR_INVALID_ARG;
     }
-    *n_launches = b->n_launches;
-    for (const auto *sh : b->shards) {
+    *n_launches = 0u;
+    for (const auto &sh : b->shards) {
         *n_launches += sh->n_launches;
     }
     return HY_OK;

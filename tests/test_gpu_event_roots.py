@@ -154,9 +154,11 @@ def test_many_candidates():
 
 
 def test_order_48_refused():
+    """The same error class on one device and on a batch made of two shards."""
     x, = hb.make_vars("x")
-    hb.taylor_adaptive_batch([(x, hb.expression(1.0))], np.zeros((1, 2)), 2, tol=5e-40,
-                             nt_events=[hb.nt_event_batch(x - 0.5, lambda ta, t, d, i: None)])
-    with pytest.raises(NotImplementedError, match="Event detection supports Taylor orders up to 47"):
-        hb.taylor_adaptive_batch([(x, hb.expression(1.0))], np.zeros((1, 2)), 2, tol=1e-40,
-                                 nt_events=[hb.nt_event_batch(x - 0.5, lambda ta, t, d, i: None)])
+    for kw in ({}, {"device": [0, 0]}):
+        hb.taylor_adaptive_batch([(x, hb.expression(1.0))], np.zeros((1, 2)), 2, tol=5e-40,
+                                 nt_events=[hb.nt_event_batch(x - 0.5, lambda ta, t, d, i: None)], **kw)
+        with pytest.raises(NotImplementedError, match="Event detection supports Taylor orders up to 47"):
+            hb.taylor_adaptive_batch([(x, hb.expression(1.0))], np.zeros((1, 2)), 2, tol=1e-40,
+                                     nt_events=[hb.nt_event_batch(x - 0.5, lambda ta, t, d, i: None)], **kw)

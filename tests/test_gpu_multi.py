@@ -110,6 +110,23 @@ def test_sharded_with_parameters_and_time():
     # (propagate_grid() and continuous output of this sharded batch: tests/test_zz_gpu_late_additions.py)
 
 
+def test_sharded_step_refuses_nan_limit_before_any_shard_steps():
+    """A NaN max_delta_t in the last shard's lanes only is refused with the single-device message, and no lane of any
+    shard has stepped. (Through the C ABI: the front end refuses NaN limits before the library sees them.)"""
+    batch = 10
+    P = hb.Program(sys_outer_ss(), high_accuracy=True)
+    b = hb.Batch(P, batch, device=[0, 0, 0])  # lanes [0, 4), [4, 7), [7, 10)
+    z = np.zeros(batch)
+    b.upload(outer_ss_batch_state(batch), None, z, z)
+    before = b.download()
+    mdt = np.full(batch, 0.1)
+    mdt[8] = np.nan
+    with pytest.raises(ValueError, match=r"Cannot use a nan max_delta_t in the step\(\) function"):
+        b.step(mdt)
+    for x, y in zip(before, b.download()):
+        assert np.array_equal(x, y)
+
+
 @pytest.mark.parametrize("devs", [None, [0, 0, 0]] + ([[0, 1]] if hb.lib.hy_device_count() >= 2 else []))
 def test_propagate_until_host_one_call(devs):
     """hy_batch_propagate_until_host(): upload + propagate_until + downloads in one call, on one device, on one device in

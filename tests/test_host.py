@@ -128,6 +128,28 @@ def test_no_cpu_fallback_without_device():
     assert "HYERROR -3" in out and "no CPU fallback" in out
 
 
+def test_null_batch_handle_is_an_invalid_argument():
+    """Every hy_batch_* function that takes a batch handle and returns a status code refuses a NULL handle with
+    HY_ERR_INVALID_ARG, before it touches a device (run in a subprocess without a device, so that a crash is a failure
+    rather than the end of the test run)."""
+    import subprocess
+    import sys
+    hdr = open(os.path.join(ROOT, "include", "heyoka_b200.h")).read()
+    names = sorted(set(re.findall(r"\bint\s+(hy_batch_[a-z0-9_]+)\s*\(\s*(?:const\s+)?hy_batch\s*\*", hdr)))
+    assert len(names) >= 29
+    code = ("import ctypes as C\n"
+            "from heyoka_b200 import _capi\n"
+            "ints = (C.c_int, C.c_uint32, C.c_int64, C.c_uint64)\n"
+            "for name in %r:\n"
+            "    args = [0. if t is C.c_double else 0 if t in ints else None for t in _capi.SIGNATURES[name][1]]\n"
+            "    print(name, getattr(_capi.lib, name)(*args), flush=True)\n" % (names,))
+    env = dict(os.environ, CUDA_VISIBLE_DEVICES="", PYTHONPATH=ROOT)
+    res = subprocess.run([sys.executable, "-c", code], env=env, capture_output=True, text=True)
+    got = dict(line.split() for line in res.stdout.splitlines())
+    assert res.returncode == 0, (res.returncode, sorted(set(names) - set(got)), res.stderr[-2000:])
+    assert got == {n: str(_capi.HY_ERR_INVALID_ARG) for n in names}
+
+
 def test_model_builders_decomposition_pinned():
     """heyoka_b200/csrc/model.cpp was rewritten in round 2 (table-driven pair enumeration, layer builder over index
     ranges): the expression trees - hence the Taylor decompositions - must be exactly what they were (hashes of
