@@ -73,7 +73,7 @@ enum nb_phase : int {
     NB_PH_PAIR,      // pair_block() of an order pair, and the sync after it
     NB_PH_SUM,       // the summation rounds of an order pair and their syncs
     NB_PH_INIT,      // role_init(): order 0 from the state, and the sync after it
-    NB_PH_STEP_SIZE, // nb_step_size() on the owner threads, and the sync after it
+    NB_PH_STEP_SIZE, // the step size (norm reduction, nb_step_size() or nb_rho()), and the sync after it
     NB_PH_UPDATE,    // coop_update_state() and the reduction of its non-finite mask
     NB_PH_PROP,      // the lane_prop bookkeeping, the loop test and chunk changes
     NB_PH_STEPS,     // (count of warp-steps)
@@ -198,6 +198,9 @@ __device__ __forceinline__ d2 from_words(std::uint32_t a, std::uint32_t b, std::
 template <int TT, bool OFFCHIP>
 struct pair_mem {
     static constexpr int NSR = OFFCHIP ? 2 : 5;
+    // pair_block()'s reciprocals ahead of the main loop (nb_core.hpp, early_den()): not with the rows off chip, where
+    // the reload of r2^[0]'s terms is an L2 access and the 512-thread kernel has no registers to spare.
+    static constexpr bool EARLY_DEN = !OFFCHIP;
     static constexpr std::uint32_t OPB = static_cast<std::uint32_t>(NSR) * TT * 16u; // bytes per order pair
     static constexpr std::uint32_t RB = TT * 16u;                                    // bytes per row
     std::uint32_t pa[3], pb[3]; // the six positions this pair reads (this thread's lane)
@@ -542,6 +545,14 @@ static __device__ __noinline__ double nb_step_size(double inv_p, double inv_pm1,
     return h_from_norms(inv_p, inv_pm1, rhofac, isnan(f0) ? f0 : m0, isnan(fp) ? fp : mp, isnan(fp1) ? fp1 : mp1,
                         max_delta_t);
 }
+// One of the two radii of convergence of nb_step_size() (order p: inv = 1 / p, order p - 1: inv = 1 / (p - 1)) from the
+// maxima m0 (order 0) and m (that order), with the same NaN rule: c0, c = the coefficients of state variable 0 at
+// order 0 and at that order. Out of line: one copy of pow() in the kernel.
+static __device__ __noinline__ double nb_rho(double inv, double m0, double m, double c0, double c)
+{
+    const double f0 = fabs(c0), f = fabs(c);
+    return rho_from_norm(isnan(f0) ? f0 : m0, isnan(f) ? f : m, inv);
+}
 
 // LT: lanes per team; CTA: a team is the whole CTA (else a warp); OFFCHIP: r^2, d_2, r^alpha rows in NP.offchip.
 template <int LT, bool CTA, bool OFFCHIP, bool PROP, int MAXT>
@@ -728,16 +739,37 @@ __global__ void __launch_bounds__(MAXT, 1) k_nb(program P, nb_dev_plan NP, batch
             }
             clk.lap(NB_PH_SUM);
         }
-        if constexpr (REGN) {
-            RM.template norms_reduce<LT>(tid, nm3);
-        }
     };
 
-    // Step size from the norms gathered during the jet (owner threads: one lane each); resets the norms.
-    const auto step_size = [&](std::uint32_t lane, double max_delta_t) {
-        const double *c = cv.base + cv.lane_off(lane, tid);
-        return nb_step_size(P.inv_p, P.inv_pm1, P.rhofac, REGN ? nullptr : norms_p + tid, LT, nm3[0], nm3[1], nm3[2], c,
-                            p * cv.stride_o, (p - 1u) * cv.stride_o, max_delta_t);
+    // Step size from the norms gathered during the jet; resets the norms. Every thread of the team calls it; the owner
+    // threads get the step size of their lane.
+    // PAIRED (warp teams of at most 16 lanes with the maxima in registers): the two radii of convergence of a lane are
+    // computed side by side, the order-p one by the lane's owner tid and the order-(p - 1) one by thread tid + LT, in
+    // the same instructions; a shuffle brings the second to the owner. The coefficients of state variable 0 that the
+    // NaN rule reads are loaded before the shuffle reduction of the maxima, which hides their latency.
+    constexpr bool PAIRED = REGN && 2 * LT <= 32;
+    const auto step_size = [&](std::uint32_t lane0, double max_delta_t) {
+        const std::uint32_t o = PAIRED ? tid % LT : tid; // the lane's owner
+        const std::uint32_t lane_raw = lane0 + o, lane = lane_raw < D.n ? lane_raw : D.n - 1u;
+        const double *c = cv.base + cv.lane_off(lane, o);
+        if constexpr (PAIRED) {
+            const bool ord_p = owner; // (threads beyond 2 LT repeat the order-(p - 1) radius of their lane)
+            const double c0 = c[0], cq = c[(ord_p ? p : p - 1u) * cv.stride_o];
+            RM.template norms_reduce<LT>(tid, nm3);
+            const double rho = nb_rho(ord_p ? P.inv_p : P.inv_pm1, nm3[0], ord_p ? nm3[1] : nm3[2], c0, cq);
+            const double rho_m1 = __shfl_down_sync(0xffffffffu, rho, LT);
+            return h_from_rho(rho, rho_m1, P.rhofac, max_delta_t);
+        } else {
+            if constexpr (REGN) {
+                RM.template norms_reduce<LT>(tid, nm3);
+            }
+            double h = 0.;
+            if (owner) {
+                h = nb_step_size(P.inv_p, P.inv_pm1, P.rhofac, REGN ? nullptr : norms_p + tid, LT, nm3[0], nm3[1],
+                                 nm3[2], c, p * cv.stride_o, (p - 1u) * cv.stride_o, max_delta_t);
+            }
+            return h;
+        }
     };
     if (owner) {
         for (std::uint32_t i = 0; i < 3u * NC; ++i) {
@@ -765,10 +797,12 @@ __global__ void __launch_bounds__(MAXT, 1) k_nb(program P, nb_dev_plan NP, batch
             }
             T::sync();
             jet(lane0);
-            double h = 0., mdt = 0.;
+            double mdt = 0.;
             if (owner) {
                 mdt = R.max_delta_t != nullptr ? R.max_delta_t[lane] : R.default_max_delta_t;
-                h = step_size(lane, mdt);
+            }
+            const double h = step_size(lane0, mdt);
+            if (owner) {
                 S.h[tid] = h;
             }
             T::sync();
@@ -801,10 +835,12 @@ __global__ void __launch_bounds__(MAXT, 1) k_nb(program P, nb_dev_plan NP, batch
                 clk.lap(NB_PH_PROP);
                 clk.step();
                 jet(lane0);
-                double h = 0., cur_max = 0.;
+                double cur_max = 0.;
                 if (owner) {
                     cur_max = park->cur_max();
-                    h = step_size(lane, cur_max);
+                }
+                const double h = step_size(lane0, cur_max);
+                if (owner) {
                     S.h[tid] = h;
                 }
                 T::sync();

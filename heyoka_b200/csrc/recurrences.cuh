@@ -657,6 +657,20 @@ __device__ __forceinline__ double std_min(double a, double b)
     return (b < a) ? b : a;
 }
 
+// The two halves of h_from_norms(), for callers that compute the two radii apart: one radius of convergence,
+// (num_rho / m)^inv with num_rho = max(1, m0), and the step size from the radii of the orders p and p - 1.
+__device__ __forceinline__ double rho_from_norm(double m0, double m, double inv)
+{
+    const double num_rho = (m0 <= 1.) ? 1. : m0;
+    return ::pow(num_rho / m, inv);
+}
+__device__ __forceinline__ double h_from_rho(double rho_o, double rho_om1, double rhofac, double max_delta_t)
+{
+    const double rho_m = std_min(rho_o, rho_om1);
+    double h = rho_m * rhofac;
+    h = std_min(h, fabs(max_delta_t));
+    return (max_delta_t < 0.) ? -h : h;
+}
 // taylor_determine_h() (src/taylor_00.cpp:102-273) from the three infinity norms: Jorba-Zou step size,
 // clamped to |max_delta_t|, signed like max_delta_t.
 // (The program's three constants as values: for out-of-line callers, which would otherwise copy the program to
@@ -664,13 +678,7 @@ __device__ __forceinline__ double std_min(double a, double b)
 __device__ __forceinline__ double h_from_norms(double inv_p, double inv_pm1, double rhofac, double m0, double mp,
                                                double mp1, double max_delta_t)
 {
-    const double num_rho = (m0 <= 1.) ? 1. : m0;
-    const double rho_o = ::pow(num_rho / mp, inv_p);
-    const double rho_om1 = ::pow(num_rho / mp1, inv_pm1);
-    const double rho_m = std_min(rho_o, rho_om1);
-    double h = rho_m * rhofac;
-    h = std_min(h, fabs(max_delta_t));
-    return (max_delta_t < 0.) ? -h : h;
+    return h_from_rho(rho_from_norm(m0, mp, inv_p), rho_from_norm(m0, mp1, inv_pm1), rhofac, max_delta_t);
 }
 __device__ __forceinline__ double h_from_norms(const program &P, double m0, double mp, double mp1, double max_delta_t)
 {
