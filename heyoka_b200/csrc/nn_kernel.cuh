@@ -17,7 +17,13 @@
 // The Taylor coefficients of the state variables live in shared memory too (step size, state update, optional copy to
 // the public tc array): apart from state in / state out nothing touches HBM.
 // Only the matrix products differ from the generic kernels (same products, different association, fused): a few ulp on
-// every z^[n] (tests/test_gpu_parity.py::test_ffnn_parity states the bound).
+// every z^[n] (tests/test_gpu_nn_shapes.py states the bound against a series reference of the network).
+// Divergence from the reference on non-finite states: the matrix product multiplies the zero weights too, and
+// 0 * NaN = NaN, whereas the reference never multiplies by a weight the expression builder dropped. So a NaN (or inf)
+// in one state variable of a lane reaches every neuron of that lane, every state variable's coefficients of order >= 1,
+// its step size and its time. The generic kernels keep the NaN in the state variables whose jet reads it, and their
+// step size stays finite unless state variable 0 is one of them. The lane's outcome (err_nf_state) and every other lane
+// are the same (tests/test_gpu_nn_shapes.py::test_one_product_nan_lane_in_last_cta).
 #ifndef HEYOKA_B200_CSRC_NN_KERNEL_CUH
 #define HEYOKA_B200_CSRC_NN_KERNEL_CUH
 

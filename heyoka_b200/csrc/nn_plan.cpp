@@ -80,6 +80,20 @@ nn_plan make_nn_plan(const hy_program &p)
                 case HY_OP_NEG:
                     expand(op.a, -scale, lf);
                     break;
+                // Weights of +-1 are folded into plain variables and negations, and the sums that hold them into
+                // differences: x - y, x - b, b - x.
+                case HY_OP_SUB_VV:
+                    expand(op.a, scale, lf);
+                    expand(op.b, -scale, lf);
+                    break;
+                case HY_OP_SUB_VN:
+                    expand(op.a, scale, lf);
+                    lf.bias -= scale * p.consts[op.b];
+                    break;
+                case HY_OP_SUB_NV:
+                    lf.bias += scale * p.consts[op.a];
+                    expand(op.b, -scale, lf);
+                    break;
                 default:
                     throw fail{"a neuron contains opcode " + std::to_string(op.opcode)};
             }

@@ -2,7 +2,8 @@
 //
 // A program qualifies when its right-hand side is a feed-forward network of dense layers, x' = ffnn(x)
 // (src/model/ffnn.cpp:36-142): after decomposition every neuron is a (nested, <= 8 terms per node: src/math/sum.cpp)
-// sum of products w_ij * in_j plus a bias, followed by tanh (with its hidden dependency tanh^2, src/math/tanh.cpp) or,
+// sum of products w_ij * in_j plus a bias (weights of +-1 folded into plain inputs, negations and differences),
+// followed by tanh (with its hidden dependency tanh^2, src/math/tanh.cpp) or,
 // for the output layer, by nothing. The planner walks those sums back into what they are - one weight matrix and one
 // bias vector per layer - so that the device can evaluate a layer of every Taylor order as ONE matrix product
 // [n_out x n_in] . [n_in x lanes] on the FP64 tensor cores (mma.sync.m8n8k4.f64) instead of interpreting ~10^4 products
