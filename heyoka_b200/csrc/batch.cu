@@ -1206,6 +1206,24 @@ struct device_guard {
     }
 };
 
+// Device memory freed when its owner goes.
+struct cuda_free {
+    void operator()(void *p) const noexcept
+    {
+        cudaFree(p);
+    }
+};
+template <typename T>
+using dev_ptr = std::unique_ptr<T, cuda_free>;
+
+template <typename T>
+dev_ptr<T> dev_alloc(std::size_t count)
+{
+    void *p = nullptr;
+    HY_CUDA_CHECK(cudaMalloc(&p, sizeof(T) * count));
+    return dev_ptr<T>(static_cast<T *>(p));
+}
+
 // The device state of `lanes` lanes of the program on `device`.
 std::unique_ptr<shard> make_shard(const hy_program &p, std::uint32_t lanes, int device)
 {
@@ -2127,7 +2145,7 @@ int hy_batch_propagate_until_dev(hy_batch *b, const double *d_t_final_hi, const 
 // propagate_grid() (src/taylor_adaptive_batch.cpp:1545-2055). The reference's algorithm is kept as it is: an
 // initial propagate_until(grid[0]) with write_tc, then lock-step iterations of {dense output at every grid point
 // covered by the last step; one step clamped to the last grid point}. The per-lane work runs on the device (one
-// step launch + two small kernels per iteration); the host only reads the two loop flags.
+// step launch + three small kernels per iteration); the host only reads the loop flags.
 namespace
 {
 
@@ -2206,6 +2224,72 @@ void check_grid(hy_batch *b, const double *grid, uint64_t n_pts, const double *m
     }
 }
 
+// The reference's lock-step loop (src/taylor_adaptive_batch.cpp:1372-1527, :1696-2053) as propagate_grid() and
+// propagate_until() with continuous output run it: the per-lane state of dev::lockstep_state and the buffers behind it.
+// An iteration is iterate(), whatever the caller launches after the bookkeeping, then read(): one read-back per
+// iteration.
+struct lockstep {
+    shard &sh;
+    dev_ptr<double> lane; // rem_hi, rem_lo, dt_limit, max_delta_t: [4][n]
+    dev_ptr<unsigned char> dir;
+    dev_ptr<unsigned> d_flags; // [0, 3) those of dev::lockstep_state, [3] one more word for the caller
+    dev::lockstep_state L{};
+    unsigned flags[4] = {0u, 0u, 0u, 0u}; // as last read back
+
+    // d_tf_hi, d_tf_lo: the target times on the device (d_tf_lo may be null); max_delta_t: host array or null.
+    lockstep(shard &s, const double *d_tf_hi, const double *d_tf_lo, const double *max_delta_t)
+        : sh(s), lane(dev_alloc<double>(4u * std::size_t(s.n))), dir(dev_alloc<unsigned char>(s.n)),
+          d_flags(dev_alloc<unsigned>(4u))
+    {
+        const std::uint32_t n = sh.n;
+        if (max_delta_t != nullptr) {
+            HY_CUDA_CHECK(cudaMemcpyAsync(lane.get() + 3u * n, max_delta_t, sizeof(double) * n, cudaMemcpyHostToDevice,
+                                          sh.stream));
+        }
+        L.tf_hi = d_tf_hi;
+        L.tf_lo = d_tf_lo;
+        L.max_delta_t = max_delta_t != nullptr ? lane.get() + 3u * n : nullptr;
+        L.rem_hi = lane.get();
+        L.rem_lo = lane.get() + n;
+        L.dt_limit = lane.get() + 2u * n;
+        L.t_dir = dir.get();
+        L.flags = d_flags.get();
+    }
+    unsigned blocks() const
+    {
+        return (sh.n + 127u) / 128u;
+    }
+    // Remaining times, directions, counters and the limit of the first step.
+    void init()
+    {
+        HY_CUDA_CHECK(cudaMemsetAsync(d_flags.get(), 0, sizeof(flags), sh.stream));
+        dev::k_lockstep_init<<<blocks(), 128, 0, sh.stream>>>(sh.view(), L, sh.d_prop_min_h, sh.d_prop_max_h,
+                                                                sh.d_prop_n_steps);
+        HY_CUDA_CHECK(cudaGetLastError());
+    }
+    // One step of every lane within its dt_limit, with its Taylor coefficients written to sh.d_tc, then the
+    // bookkeeping. All four flag words start the iteration cleared.
+    void iterate()
+    {
+        dev::run_args R{};
+        R.max_delta_t = L.dt_limit;
+        R.default_max_delta_t = std::numeric_limits<double>::infinity();
+        R.write_tc = 1;
+        R.flags = sh.d_flags;
+        R.counter = sh.d_counter;
+        sh.launch(false, R);
+        HY_CUDA_CHECK(cudaMemsetAsync(d_flags.get(), 0, sizeof(flags), sh.stream));
+        dev::k_lockstep_book<<<blocks(), 128, 0, sh.stream>>>(sh.view(), L, sh.d_prop_outcome, sh.d_prop_min_h,
+                                                                sh.d_prop_max_h, sh.d_prop_n_steps);
+        HY_CUDA_CHECK(cudaGetLastError());
+    }
+    void read()
+    {
+        HY_CUDA_CHECK(cudaMemcpyAsync(flags, d_flags.get(), sizeof(flags), cudaMemcpyDeviceToHost, sh.stream));
+        HY_CUDA_CHECK(cudaStreamSynchronize(sh.stream));
+    }
+};
+
 } // namespace
 
 int hy_batch_check_grid(hy_batch *b, const double *grid, uint64_t n_pts, const double *max_delta_t)
@@ -2224,18 +2308,6 @@ int hy_batch_check_grid(hy_batch *b, const double *grid, uint64_t n_pts, const d
 int hy_batch_propagate_grid(hy_batch *b, const double *grid, uint64_t n_pts, const double *max_delta_t,
                             uint64_t max_steps, double *out)
 {
-    double *d_grid = nullptr, *d_out = nullptr, *d_lane = nullptr;
-    std::uint32_t *d_idx = nullptr;
-    unsigned char *d_dir = nullptr;
-    unsigned *d_gflags = nullptr;
-    const auto cleanup = [&]() {
-        for (void *ptr : {static_cast<void *>(d_grid), static_cast<void *>(d_out), static_cast<void *>(d_lane),
-                          static_cast<void *>(d_idx), static_cast<void *>(d_dir), static_cast<void *>(d_gflags)}) {
-            if (ptr != nullptr) {
-                cudaFree(ptr);
-            }
-        }
-    };
     try {
         refuse_events(b);
         if (b == nullptr || grid == nullptr || out == nullptr) {
@@ -2250,32 +2322,25 @@ int hy_batch_propagate_grid(hy_batch *b, const double *grid, uint64_t n_pts, con
         const std::uint32_t n = sh.n;
 
         const std::size_t n_out = static_cast<std::size_t>(n_pts) * sh.n_eq * n, state_doubles = std::size_t(sh.n_eq) * n;
-        HY_CUDA_CHECK(cudaMalloc(&d_grid, sizeof(double) * n_pts * n));
-        HY_CUDA_CHECK(cudaMalloc(&d_out, sizeof(double) * n_out));
-        HY_CUDA_CHECK(cudaMalloc(&d_lane, sizeof(double) * 4u * n)); // rem_hi, rem_lo, dt_limit, max_delta_t
-        HY_CUDA_CHECK(cudaMalloc(&d_idx, sizeof(std::uint32_t) * n));
-        HY_CUDA_CHECK(cudaMalloc(&d_dir, n));
-        HY_CUDA_CHECK(cudaMalloc(&d_gflags, sizeof(unsigned) * 4u));
-        HY_CUDA_CHECK(cudaMemcpyAsync(d_grid, grid, sizeof(double) * n_pts * n, cudaMemcpyHostToDevice, sh.stream));
-        if (max_delta_t != nullptr) {
-            HY_CUDA_CHECK(cudaMemcpyAsync(d_lane + 3u * n, max_delta_t, sizeof(double) * n, cudaMemcpyHostToDevice,
-                                          sh.stream));
-        }
+        const auto d_grid = dev_alloc<double>(n_pts * n), d_out = dev_alloc<double>(n_out);
+        const auto d_idx = dev_alloc<std::uint32_t>(n);
+        HY_CUDA_CHECK(cudaMemcpyAsync(d_grid.get(), grid, sizeof(double) * n_pts * n, cudaMemcpyHostToDevice, sh.stream));
+        // The target of every lane is its last grid point.
+        lockstep ls(sh, d_grid.get() + (n_pts - 1u) * n, nullptr, max_delta_t);
         dev::k_fill_double<<<static_cast<unsigned>((n_out + 255u) / 256u), 256, 0, sh.stream>>>(
-            d_out, n_out, std::numeric_limits<double>::quiet_NaN());
+            d_out.get(), n_out, std::numeric_limits<double>::quiet_NaN());
         HY_CUDA_CHECK(cudaGetLastError());
-        const unsigned gb = (n + 127u) / 128u;
+        const unsigned gb = ls.blocks();
         const auto finish = [&]() {
-            HY_CUDA_CHECK(cudaMemcpyAsync(out, d_out, sizeof(double) * n_out, cudaMemcpyDeviceToHost, sh.stream));
+            HY_CUDA_CHECK(cudaMemcpyAsync(out, d_out.get(), sizeof(double) * n_out, cudaMemcpyDeviceToHost, sh.stream));
             HY_CUDA_CHECK(cudaStreamSynchronize(sh.stream));
-            cleanup();
             return HY_OK;
         };
 
         // Up to the first grid point (a zero-length step when the time is already there: it brings the Taylor
         // coefficients up to date), :1697-1706.
         {
-            propagate(b, d_grid, nullptr, max_delta_t != nullptr ? d_lane + 3u * n : nullptr, 1, max_steps, 1, nullptr);
+            propagate(b, d_grid.get(), nullptr, ls.L.max_delta_t, 1, max_steps, 1, nullptr);
             std::vector<long long> oc(n);
             HY_CUDA_CHECK(cudaMemcpyAsync(oc.data(), sh.d_prop_outcome, sizeof(long long) * n, cudaMemcpyDeviceToHost,
                                           sh.stream));
@@ -2288,53 +2353,34 @@ int hy_batch_propagate_grid(hy_batch *b, const double *grid, uint64_t n_pts, con
                 return finish();
             }
         }
-        HY_CUDA_CHECK(cudaMemcpyAsync(d_out, sh.d_state, sizeof(double) * state_doubles, cudaMemcpyDeviceToDevice,
+        HY_CUDA_CHECK(cudaMemcpyAsync(d_out.get(), sh.d_state, sizeof(double) * state_doubles, cudaMemcpyDeviceToDevice,
+                                      sh.stream));
+        // Grid point 0 is the state just copied: every cursor starts at 1.
+        const std::vector<std::uint32_t> first(n, 1u);
+        HY_CUDA_CHECK(cudaMemcpyAsync(d_idx.get(), first.data(), sizeof(std::uint32_t) * n, cudaMemcpyHostToDevice,
                                       sh.stream));
 
-        dev::grid_state G{};
-        G.grid = d_grid;
-        G.n_pts = static_cast<std::uint32_t>(n_pts);
-        G.out = d_out;
-        G.max_delta_t = max_delta_t != nullptr ? d_lane + 3u * n : nullptr;
-        G.cur_idx = d_idx;
-        G.rem_hi = d_lane;
-        G.rem_lo = d_lane + n;
-        G.t_dir = d_dir;
-        G.dt_limit = d_lane + 2u * n;
-        G.flags = d_gflags;
-        unsigned hflags[4] = {0u, 0u, 0u, 0u};
-        const auto read_flags = [&]() {
-            HY_CUDA_CHECK(cudaMemcpyAsync(hflags, d_gflags, sizeof(hflags), cudaMemcpyDeviceToHost, sh.stream));
-            HY_CUDA_CHECK(cudaStreamSynchronize(sh.stream));
-        };
-        HY_CUDA_CHECK(cudaMemsetAsync(d_gflags, 0, sizeof(hflags), sh.stream));
-        dev::k_grid_init<<<gb, 128, 0, sh.stream>>>(sh.view(), G, sh.d_prop_min_h, sh.d_prop_max_h, sh.d_prop_n_steps);
-        dev::k_grid_sample<<<dim3(gb, sh.n_eq), 128, 0, sh.stream>>>(sh.prog, sh.view(), G);
-        dev::k_grid_advance<<<gb, 128, 0, sh.stream>>>(sh.view(), G);
+        // The word the lock-step state leaves to its caller says whether some lane has grid points left.
+        const dev::grid_state G{d_grid.get(), static_cast<std::uint32_t>(n_pts), d_out.get(), d_idx.get(),
+                                ls.d_flags.get() + 3};
+        ls.init();
+        dev::k_grid_sample<<<dim3(gb, sh.n_eq), 128, 0, sh.stream>>>(sh.prog, sh.view(), G, ls.L);
+        dev::k_grid_advance<<<gb, 128, 0, sh.stream>>>(sh.view(), G, ls.L);
         HY_CUDA_CHECK(cudaGetLastError());
-        read_flags();
-        if (hflags[2] != 0u) {
+        ls.read();
+        if (ls.flags[2] != 0u) {
             throw std::invalid_argument("The final time passed to the propagate_grid() function of an adaptive Taylor "
                                         "integrator in batch mode results in an overflow condition");
         }
         std::uint64_t iter = 0;
         bool interrupted = false;
-        while (hflags[0] != 0u && !interrupted) {
-            dev::run_args R{};
-            R.max_delta_t = G.dt_limit;
-            R.default_max_delta_t = std::numeric_limits<double>::infinity();
-            R.write_tc = 1;
-            R.flags = sh.d_flags;
-            R.counter = sh.d_counter;
-            sh.launch(false, R);
-            HY_CUDA_CHECK(cudaMemsetAsync(d_gflags, 0, sizeof(unsigned) * 2u, sh.stream));
-            dev::k_grid_book<<<gb, 128, 0, sh.stream>>>(sh.view(), G, sh.d_prop_outcome, sh.d_prop_min_h,
-                                                         sh.d_prop_max_h, sh.d_prop_n_steps);
-            dev::k_grid_sample<<<dim3(gb, sh.n_eq), 128, 0, sh.stream>>>(sh.prog, sh.view(), G);
-            dev::k_grid_advance<<<gb, 128, 0, sh.stream>>>(sh.view(), G);
+        while (ls.flags[3] != 0u && !interrupted) {
+            ls.iterate();
+            dev::k_grid_sample<<<dim3(gb, sh.n_eq), 128, 0, sh.stream>>>(sh.prog, sh.view(), G, ls.L);
+            dev::k_grid_advance<<<gb, 128, 0, sh.stream>>>(sh.view(), G, ls.L);
             HY_CUDA_CHECK(cudaGetLastError());
-            read_flags();
-            if (hflags[1] != 0u) {
+            ls.read();
+            if (ls.flags[1] != 0u) {
                 break; // non-finite state: nothing further is written (:1973-1978)
             }
             if (++iter == max_steps) {
@@ -2345,7 +2391,6 @@ int hy_batch_propagate_grid(hy_batch *b, const double *grid, uint64_t n_pts, con
         }
         return finish();
     } catch (...) {
-        cleanup();
         return translate_exception();
     }
 }
@@ -2360,24 +2405,116 @@ struct hy_cout {
     dev::program prog{};
     // The Taylor coefficients of the recorded iterations live in slabs of slab_iters iterations each, written in
     // place by the step kernel (no copy, no final re-pack); d_slabs is the device-side table of the slab pointers.
-    std::vector<double *> slabs;
-    double **d_slabs = nullptr;
+    std::vector<dev_ptr<double>> slabs;
+    dev_ptr<double *> d_slabs;
     std::uint32_t slab_iters = 1;
     cudaStream_t stream = nullptr;
-    double *d_t_hi = nullptr, *d_t_lo = nullptr, *d_tm = nullptr, *d_out = nullptr;
-    ~hy_cout()
-    {
-        for (double *ptr : slabs) {
-            cudaFree(ptr);
-        }
-        for (void *ptr : {static_cast<void *>(d_slabs), static_cast<void *>(d_t_hi), static_cast<void *>(d_t_lo),
-                          static_cast<void *>(d_tm), static_cast<void *>(d_out)}) {
-            if (ptr != nullptr) {
-                cudaFree(ptr);
-            }
-        }
-    }
+    dev_ptr<double> d_t_hi, d_t_lo, d_tm, d_out;
 };
+
+// A recording under construction (update_c_out() / make_c_out(), src/taylor_adaptive_batch.cpp:1277-1346): the
+// Taylor coefficients of the current iteration go to slot(), commit() appends the times and closes the iteration.
+// The device loop of hy_batch_propagate_until_cout_cb() has the step kernel write straight into the slot; the front
+// ends' host lock-step loops (integrators with events, whose callbacks are host code) copy the step's tc array there
+// through hy_cout_rec_append().
+struct hy_cout_rec {
+    std::unique_ptr<hy_cout> co;
+    dev_ptr<double> d_times; // rows of 2 * n doubles (hi, lo)
+    std::size_t times_cap = 0, times_rows = 0, tc_doubles = 0;
+    std::uint64_t iter = 0; // committed iterations
+
+    explicit hy_cout_rec(shard &sh);
+    double *slot();
+    void commit(shard &sh);
+    hy_cout *finish(shard &sh, const unsigned char *forward);
+
+private:
+    void push_times(shard &sh);
+};
+
+// Row 0 of the times: the starting times.
+hy_cout_rec::hy_cout_rec(shard &sh)
+    : co(std::make_unique<hy_cout>()), tc_doubles(static_cast<std::size_t>(sh.n_eq) * (sh.order + 1u) * sh.n)
+{
+    co->device = sh.device;
+    co->n = sh.n;
+    co->n_eq = sh.n_eq;
+    co->order = sh.order;
+    co->prog = sh.prog;
+    co->stream = sh.stream;
+    // Slabs of about 64 MB (at least one iteration each).
+    co->slab_iters = static_cast<std::uint32_t>(
+        std::min<std::size_t>(std::max<std::size_t>((std::size_t(64) << 20) / (tc_doubles * sizeof(double)), 1u), 4096u));
+    push_times(sh);
+}
+
+void hy_cout_rec::push_times(shard &sh)
+{
+    const std::uint32_t n = sh.n;
+    if (times_rows == times_cap) {
+        const std::size_t new_cap = std::max<std::size_t>(2u * times_cap, 64u);
+        auto nt = dev_alloc<double>(2u * n * new_cap);
+        if (d_times != nullptr) {
+            HY_CUDA_CHECK(cudaMemcpyAsync(nt.get(), d_times.get(), sizeof(double) * 2u * n * times_rows,
+                                          cudaMemcpyDeviceToDevice, sh.stream));
+            HY_CUDA_CHECK(cudaStreamSynchronize(sh.stream));
+        }
+        d_times = std::move(nt);
+        times_cap = new_cap;
+    }
+    double *blk = d_times.get() + 2u * n * times_rows;
+    HY_CUDA_CHECK(cudaMemcpyAsync(blk, sh.d_t_hi, sizeof(double) * n, cudaMemcpyDeviceToDevice, sh.stream));
+    HY_CUDA_CHECK(cudaMemcpyAsync(blk + n, sh.d_t_lo, sizeof(double) * n, cudaMemcpyDeviceToDevice, sh.stream));
+    ++times_rows;
+}
+
+// The Taylor coefficients of the current iteration; a slab is allocated when the iteration starts one.
+double *hy_cout_rec::slot()
+{
+    if (iter / co->slab_iters == co->slabs.size()) {
+        co->slabs.push_back(dev_alloc<double>(tc_doubles * co->slab_iters));
+    }
+    return co->slabs[iter / co->slab_iters].get() + (iter % co->slab_iters) * tc_doubles;
+}
+
+void hy_cout_rec::commit(shard &sh)
+{
+    push_times(sh);
+    ++iter;
+}
+
+// make_c_out() (:1277-1317): forward[lane] != 0 for lanes integrated forwards in time (the padding row of the times is
+// +-inf by direction). Null if nothing was recorded.
+hy_cout *hy_cout_rec::finish(shard &sh, const unsigned char *forward)
+{
+    if (iter == 0u) {
+        return nullptr;
+    }
+    const std::uint32_t n = sh.n;
+    co->n_steps = iter;
+    const std::size_t rows = iter + 2u;
+    co->d_t_hi = dev_alloc<double>(rows * n);
+    co->d_t_lo = dev_alloc<double>(rows * n);
+    co->d_tm = dev_alloc<double>(n);
+    co->d_out = dev_alloc<double>(static_cast<std::size_t>(sh.n_eq) * n);
+    HY_CUDA_CHECK(cudaMemcpy2DAsync(co->d_t_hi.get(), sizeof(double) * n, d_times.get(), sizeof(double) * 2u * n,
+                                    sizeof(double) * n, iter + 1u, cudaMemcpyDeviceToDevice, sh.stream));
+    HY_CUDA_CHECK(cudaMemcpy2DAsync(co->d_t_lo.get(), sizeof(double) * n, d_times.get() + n, sizeof(double) * 2u * n,
+                                    sizeof(double) * n, iter + 1u, cudaMemcpyDeviceToDevice, sh.stream));
+    std::vector<double *> slabs(co->slabs.size());
+    std::transform(co->slabs.begin(), co->slabs.end(), slabs.begin(), [](const dev_ptr<double> &p) { return p.get(); });
+    co->d_slabs = dev_alloc<double *>(slabs.size());
+    HY_CUDA_CHECK(cudaMemcpyAsync(co->d_slabs.get(), slabs.data(), sizeof(double *) * slabs.size(), cudaMemcpyHostToDevice,
+                                  sh.stream));
+    HY_CUDA_CHECK(cudaStreamSynchronize(sh.stream));
+    std::vector<double> pad(n), zero(n, 0.);
+    for (std::uint32_t i = 0; i < n; ++i) {
+        pad[i] = forward[i] != 0 ? std::numeric_limits<double>::infinity() : -std::numeric_limits<double>::infinity();
+    }
+    HY_CUDA_CHECK(cudaMemcpy(co->d_t_hi.get() + (rows - 1u) * n, pad.data(), sizeof(double) * n, cudaMemcpyHostToDevice));
+    HY_CUDA_CHECK(cudaMemcpy(co->d_t_lo.get() + (rows - 1u) * n, zero.data(), sizeof(double) * n, cudaMemcpyHostToDevice));
+    return co.release();
+}
 
 namespace
 {
@@ -2395,26 +2532,6 @@ int hy_batch_propagate_until_cout_cb(hy_batch *b, const double *t_final_hi, cons
                                      const double *max_delta_t, uint64_t max_steps, hy_step_callback cb, void *user,
                                      hy_cout **out)
 {
-    // The recording (hy_cout) owns its device memory from the start: slabs of Taylor coefficients the step kernel
-    // writes into directly, and the times of the iterations in a geometrically grown array.
-    std::unique_ptr<hy_cout> co;
-    double *d_lane = nullptr, *d_times = nullptr, *own_tc = nullptr;
-    std::size_t times_cap = 0, times_rows = 0; // rows of 2 * n doubles (hi, lo)
-    unsigned char *d_dir = nullptr;
-    unsigned *d_pflags = nullptr;
-    bool tc_swapped = false;
-    shard *sh = nullptr;
-    const auto cleanup = [&]() {
-        if (tc_swapped) {
-            sh->d_tc = own_tc;
-        }
-        for (void *ptr : {static_cast<void *>(d_lane), static_cast<void *>(d_dir), static_cast<void *>(d_pflags),
-                          static_cast<void *>(d_times)}) {
-            if (ptr != nullptr) {
-                cudaFree(ptr);
-            }
-        }
-    };
     try {
         refuse_events(b);
         if (b != nullptr && b->multi) {
@@ -2424,231 +2541,81 @@ int hy_batch_propagate_until_cout_cb(hy_batch *b, const double *t_final_hi, cons
             throw std::invalid_argument("Null pointer passed to hy_batch_propagate_until_cout()");
         }
         *out = nullptr;
-        sh = b->shards[0].get();
-        device_guard guard(sh->device);
-        const std::uint32_t n = sh->n;
-        // Argument checks of propagate_until_impl(), src/taylor_adaptive_batch.cpp:1212-1241.
-        for (std::uint32_t i = 0; i < n; ++i) {
-            if (!std::isfinite(t_final_hi[i]) || (t_final_lo != nullptr && !std::isfinite(t_final_lo[i]))) {
-                throw std::invalid_argument("A non-finite time was passed to the propagate_until() function of an "
-                                            "adaptive Taylor integrator in batch mode");
-            }
-            if (max_delta_t != nullptr) {
-                if (std::isnan(max_delta_t[i])) {
-                    throw std::invalid_argument("A nan max_delta_t was passed to the propagate_until() function of an "
-                                                "adaptive Taylor integrator in batch mode");
-                }
-                if (max_delta_t[i] <= 0) {
-                    throw std::invalid_argument("A non-positive max_delta_t was passed to the propagate_until() "
-                                                "function of an adaptive Taylor integrator in batch mode");
-                }
-            }
-        }
-        // rem_hi, rem_lo, dt_limit, max_delta_t, tf_hi, tf_lo
-        HY_CUDA_CHECK(cudaMalloc(&d_lane, sizeof(double) * 6u * n));
-        HY_CUDA_CHECK(cudaMalloc(&d_dir, n));
-        HY_CUDA_CHECK(cudaMalloc(&d_pflags, sizeof(unsigned) * 4u));
-        HY_CUDA_CHECK(cudaMemcpyAsync(d_lane + 4u * n, t_final_hi, sizeof(double) * n, cudaMemcpyHostToDevice, sh->stream));
+        shard &sh = *b->shards[0];
+        device_guard guard(sh.device);
+        const std::uint32_t n = sh.n;
+        check_prop_args(n, t_final_hi, t_final_lo, max_delta_t);
+        const auto d_tf = dev_alloc<double>(2u * std::size_t(n)); // tf_hi, tf_lo
+        HY_CUDA_CHECK(cudaMemcpyAsync(d_tf.get(), t_final_hi, sizeof(double) * n, cudaMemcpyHostToDevice, sh.stream));
         if (t_final_lo != nullptr) {
-            HY_CUDA_CHECK(cudaMemcpyAsync(d_lane + 5u * n, t_final_lo, sizeof(double) * n, cudaMemcpyHostToDevice,
-                                          sh->stream));
+            HY_CUDA_CHECK(cudaMemcpyAsync(d_tf.get() + n, t_final_lo, sizeof(double) * n, cudaMemcpyHostToDevice,
+                                          sh.stream));
         }
-        if (max_delta_t != nullptr) {
-            HY_CUDA_CHECK(cudaMemcpyAsync(d_lane + 3u * n, max_delta_t, sizeof(double) * n, cudaMemcpyHostToDevice,
-                                          sh->stream));
-        }
-        dev::prop_state G{};
-        G.tf_hi = d_lane + 4u * n;
-        G.tf_lo = t_final_lo != nullptr ? d_lane + 5u * n : nullptr;
-        G.max_delta_t = max_delta_t != nullptr ? d_lane + 3u * n : nullptr;
-        G.rem_hi = d_lane;
-        G.rem_lo = d_lane + n;
-        G.t_dir = d_dir;
-        G.dt_limit = d_lane + 2u * n;
-        G.flags = d_pflags;
-        const unsigned gb = (n + 127u) / 128u;
-        const std::size_t tc_doubles = static_cast<std::size_t>(sh->n_eq) * (sh->order + 1u) * n;
-        unsigned hflags[4] = {0u, 0u, 0u, 0u};
-        const auto read_flags = [&]() {
-            HY_CUDA_CHECK(cudaMemcpyAsync(hflags, d_pflags, sizeof(hflags), cudaMemcpyDeviceToHost, sh->stream));
-            HY_CUDA_CHECK(cudaStreamSynchronize(sh->stream));
-        };
-        co = std::make_unique<hy_cout>();
-        co->device = sh->device;
-        co->n = n;
-        co->n_eq = sh->n_eq;
-        co->order = sh->order;
-        co->prog = sh->prog;
-        co->stream = sh->stream;
-        // Slabs of about 64 MB (at least one iteration each).
-        co->slab_iters = static_cast<std::uint32_t>(
-            std::min<std::size_t>(std::max<std::size_t>((std::size_t(64) << 20) / (tc_doubles * sizeof(double)), 1u), 4096u));
-        // Row 0 of the times: the starting time.
-        const auto push_times = [&]() {
-            if (times_rows == times_cap) {
-                const std::size_t new_cap = std::max<std::size_t>(2u * times_cap, 64u);
-                double *nt = nullptr;
-                HY_CUDA_CHECK(cudaMalloc(&nt, sizeof(double) * 2u * n * new_cap));
-                if (d_times != nullptr) {
-                    HY_CUDA_CHECK(cudaMemcpyAsync(nt, d_times, sizeof(double) * 2u * n * times_rows, cudaMemcpyDeviceToDevice,
-                                                  sh->stream));
-                    HY_CUDA_CHECK(cudaStreamSynchronize(sh->stream));
-                    HY_CUDA_CHECK(cudaFree(d_times));
-                }
-                d_times = nt;
-                times_cap = new_cap;
+        lockstep ls(sh, d_tf.get(), t_final_lo != nullptr ? d_tf.get() + n : nullptr, max_delta_t);
+        hy_cout_rec rec(sh);
+        // The step kernel writes the coefficients of every iteration straight into their slot of the recording; the
+        // batch's own tc array is put back however the loop ends.
+        sh.ensure_tc();
+        struct tc_restore {
+            shard &sh;
+            double *const own;
+            ~tc_restore()
+            {
+                sh.d_tc = own;
             }
-            double *blk = d_times + 2u * n * times_rows;
-            HY_CUDA_CHECK(cudaMemcpyAsync(blk, sh->d_t_hi, sizeof(double) * n, cudaMemcpyDeviceToDevice, sh->stream));
-            HY_CUDA_CHECK(cudaMemcpyAsync(blk + n, sh->d_t_lo, sizeof(double) * n, cudaMemcpyDeviceToDevice, sh->stream));
-            ++times_rows;
-        };
-        push_times();
-        sh->ensure_tc();
-        own_tc = sh->d_tc;
-        tc_swapped = true;
-        HY_CUDA_CHECK(cudaMemsetAsync(d_pflags, 0, sizeof(hflags), sh->stream));
-        dev::k_prop_init<<<gb, 128, 0, sh->stream>>>(sh->view(), G, sh->d_prop_min_h, sh->d_prop_max_h, sh->d_prop_n_steps);
-        HY_CUDA_CHECK(cudaGetLastError());
-        read_flags();
-        if (hflags[2] != 0u) {
+        } tc{sh, sh.d_tc};
+        ls.init();
+        ls.read();
+        if (ls.flags[2] != 0u) {
             throw std::invalid_argument("The final time passed to the propagate_until() function of an adaptive "
                                         "Taylor integrator in batch mode results in an overflow condition");
         }
-        std::uint64_t iter = 0;
         while (true) {
-            // The step kernel writes the coefficients of this iteration straight into their slot of the recording.
-            if (iter / co->slab_iters == co->slabs.size()) {
-                double *slab = nullptr;
-                HY_CUDA_CHECK(cudaMalloc(&slab, sizeof(double) * tc_doubles * co->slab_iters));
-                co->slabs.push_back(slab);
-            }
-            sh->d_tc = co->slabs[iter / co->slab_iters] + (iter % co->slab_iters) * tc_doubles;
-            dev::run_args R{};
-            R.max_delta_t = G.dt_limit;
-            R.default_max_delta_t = std::numeric_limits<double>::infinity();
-            R.write_tc = 1;
-            R.flags = sh->d_flags;
-            R.counter = sh->d_counter;
-            sh->launch(false, R);
-            HY_CUDA_CHECK(cudaMemsetAsync(d_pflags, 0, sizeof(unsigned) * 2u, sh->stream));
-            dev::k_prop_book<<<gb, 128, 0, sh->stream>>>(sh->view(), G, sh->d_prop_outcome, sh->d_prop_min_h,
-                                                         sh->d_prop_max_h, sh->d_prop_n_steps);
-            HY_CUDA_CHECK(cudaGetLastError());
-            read_flags();
-            if (hflags[1] != 0u) {
+            sh.d_tc = rec.slot();
+            ls.iterate();
+            ls.read();
+            if (ls.flags[1] != 0u) {
                 break; // non-finite state: this iteration is not recorded (:1462-1467)
             }
-            // update_c_out(), :1320-1346.
-            push_times();
-            ++iter;
+            rec.commit(sh); // update_c_out(), :1320-1346
             if (cb != nullptr) {
                 // The step callback (:1476-1500), before the exit tests like in the reference.
-                HY_CUDA_CHECK(cudaStreamSynchronize(sh->stream));
+                HY_CUDA_CHECK(cudaStreamSynchronize(sh.stream));
                 const int r = cb(user);
                 if (r < 0) {
                     throw callback_abort{};
                 }
                 if (r == 0) {
-                    dev::k_fill_outcome<<<(n + 255u) / 256u, 256, 0, sh->stream>>>(sh->d_prop_outcome, n,
+                    dev::k_fill_outcome<<<(n + 255u) / 256u, 256, 0, sh.stream>>>(sh.d_prop_outcome, n,
                                                                                   HY_OUTCOME_CB_STOP);
                     break;
                 }
             }
-            if (hflags[0] == n) {
+            if (ls.flags[0] == n) {
                 break; // every lane reached its final time
             }
-            if (iter == max_steps) {
-                dev::k_fill_outcome<<<(n + 255u) / 256u, 256, 0, sh->stream>>>(sh->d_prop_outcome, n,
+            if (rec.iter == max_steps) {
+                dev::k_fill_outcome<<<(n + 255u) / 256u, 256, 0, sh.stream>>>(sh.d_prop_outcome, n,
                                                                               HY_OUTCOME_STEP_LIMIT);
                 break;
             }
         }
         // The batch's own tc array ends up with the coefficients of the last step taken, like m_tc in the reference.
-        HY_CUDA_CHECK(cudaMemcpyAsync(own_tc, sh->d_tc, sizeof(double) * tc_doubles, cudaMemcpyDeviceToDevice, sh->stream));
-        sh->d_tc = own_tc;
-        tc_swapped = false;
-        if (iter != 0u) {
-            // make_c_out(), :1277-1317: the times get a padding row, +-inf by direction.
-            co->n_steps = iter;
-            const std::size_t rows = iter + 2u;
-            HY_CUDA_CHECK(cudaMalloc(&co->d_t_hi, sizeof(double) * rows * n));
-            HY_CUDA_CHECK(cudaMalloc(&co->d_t_lo, sizeof(double) * rows * n));
-            HY_CUDA_CHECK(cudaMalloc(&co->d_tm, sizeof(double) * n));
-            HY_CUDA_CHECK(cudaMalloc(&co->d_out, sizeof(double) * static_cast<std::size_t>(sh->n_eq) * n));
-            HY_CUDA_CHECK(cudaMemcpy2DAsync(co->d_t_hi, sizeof(double) * n, d_times, sizeof(double) * 2u * n,
-                                            sizeof(double) * n, iter + 1u, cudaMemcpyDeviceToDevice, sh->stream));
-            HY_CUDA_CHECK(cudaMemcpy2DAsync(co->d_t_lo, sizeof(double) * n, d_times + n, sizeof(double) * 2u * n,
-                                            sizeof(double) * n, iter + 1u, cudaMemcpyDeviceToDevice, sh->stream));
-            HY_CUDA_CHECK(cudaMalloc(&co->d_slabs, sizeof(double *) * co->slabs.size()));
-            HY_CUDA_CHECK(cudaMemcpyAsync(co->d_slabs, co->slabs.data(), sizeof(double *) * co->slabs.size(),
-                                          cudaMemcpyHostToDevice, sh->stream));
-            std::vector<unsigned char> dir(n);
-            HY_CUDA_CHECK(cudaMemcpyAsync(dir.data(), d_dir, n, cudaMemcpyDeviceToHost, sh->stream));
-            HY_CUDA_CHECK(cudaStreamSynchronize(sh->stream));
-            std::vector<double> pad(n), zero(n, 0.);
-            for (std::uint32_t i = 0; i < n; ++i) {
-                pad[i] = dir[i] != 0 ? std::numeric_limits<double>::infinity() : -std::numeric_limits<double>::infinity();
-            }
-            HY_CUDA_CHECK(cudaMemcpy(co->d_t_hi + (rows - 1u) * n, pad.data(), sizeof(double) * n, cudaMemcpyHostToDevice));
-            HY_CUDA_CHECK(cudaMemcpy(co->d_t_lo + (rows - 1u) * n, zero.data(), sizeof(double) * n, cudaMemcpyHostToDevice));
-            *out = co.release();
-        }
-        HY_CUDA_CHECK(cudaStreamSynchronize(sh->stream));
-        cleanup();
+        HY_CUDA_CHECK(cudaMemcpyAsync(tc.own, sh.d_tc, sizeof(double) * rec.tc_doubles, cudaMemcpyDeviceToDevice,
+                                      sh.stream));
+        std::vector<unsigned char> forward(n);
+        HY_CUDA_CHECK(cudaMemcpyAsync(forward.data(), ls.L.t_dir, n, cudaMemcpyDeviceToHost, sh.stream));
+        HY_CUDA_CHECK(cudaStreamSynchronize(sh.stream));
+        *out = rec.finish(sh, forward.data());
+        HY_CUDA_CHECK(cudaStreamSynchronize(sh.stream));
         return HY_OK;
     } catch (const callback_abort &) {
-        cleanup();
         hy::detail::set_last_error("A host callback aborted the propagation");
         return HY_ERR_CALLBACK;
     } catch (...) {
-        cleanup();
         return translate_exception();
     }
 }
-
-// A recording driven from OUTSIDE the library: the front ends' host lock-step loops (integrators with events, whose
-// callbacks are host code: src/taylor_adaptive_batch.cpp:1372-1527 with update_c_out() at :1320-1346) append the Taylor
-// coefficients and times of every iteration they complete.
-struct hy_cout_rec {
-    std::unique_ptr<hy_cout> co;
-    double *d_times = nullptr; // rows of 2 * n doubles (hi, lo)
-    std::size_t times_cap = 0, times_rows = 0, tc_doubles = 0;
-    std::uint64_t iter = 0;
-    ~hy_cout_rec()
-    {
-        if (d_times != nullptr) {
-            cudaFree(d_times);
-        }
-    }
-};
-
-namespace
-{
-
-void rec_push_times(shard &sh, hy_cout_rec *r)
-{
-    const std::uint32_t n = sh.n;
-    if (r->times_rows == r->times_cap) {
-        const std::size_t new_cap = std::max<std::size_t>(2u * r->times_cap, 64u);
-        double *nt = nullptr;
-        HY_CUDA_CHECK(cudaMalloc(&nt, sizeof(double) * 2u * n * new_cap));
-        if (r->d_times != nullptr) {
-            HY_CUDA_CHECK(cudaMemcpyAsync(nt, r->d_times, sizeof(double) * 2u * n * r->times_rows, cudaMemcpyDeviceToDevice,
-                                          sh.stream));
-            HY_CUDA_CHECK(cudaStreamSynchronize(sh.stream));
-            HY_CUDA_CHECK(cudaFree(r->d_times));
-        }
-        r->d_times = nt;
-        r->times_cap = new_cap;
-    }
-    double *blk = r->d_times + 2u * n * r->times_rows;
-    HY_CUDA_CHECK(cudaMemcpyAsync(blk, sh.d_t_hi, sizeof(double) * n, cudaMemcpyDeviceToDevice, sh.stream));
-    HY_CUDA_CHECK(cudaMemcpyAsync(blk + n, sh.d_t_lo, sizeof(double) * n, cudaMemcpyDeviceToDevice, sh.stream));
-    ++r->times_rows;
-}
-
-} // namespace
 
 int hy_cout_rec_begin(hy_batch *b, hy_cout_rec **out)
 {
@@ -2662,18 +2629,7 @@ int hy_cout_rec_begin(hy_batch *b, hy_cout_rec **out)
         *out = nullptr;
         shard &sh = *b->shards[0];
         device_guard guard(sh.device);
-        auto r = std::make_unique<hy_cout_rec>();
-        r->tc_doubles = static_cast<std::size_t>(sh.n_eq) * (sh.order + 1u) * sh.n;
-        r->co = std::make_unique<hy_cout>();
-        r->co->device = sh.device;
-        r->co->n = sh.n;
-        r->co->n_eq = sh.n_eq;
-        r->co->order = sh.order;
-        r->co->prog = sh.prog;
-        r->co->stream = sh.stream;
-        r->co->slab_iters = static_cast<std::uint32_t>(std::min<std::size_t>(
-            std::max<std::size_t>((std::size_t(64) << 20) / (r->tc_doubles * sizeof(double)), 1u), 4096u));
-        rec_push_times(sh, r.get()); // row 0: the starting time
+        auto r = std::make_unique<hy_cout_rec>(sh);
         HY_CUDA_CHECK(cudaStreamSynchronize(sh.stream));
         *out = r.release();
         return HY_OK;
@@ -2692,17 +2648,10 @@ int hy_cout_rec_append(hy_batch *b, hy_cout_rec *r)
         }
         shard &sh = *b->shards[0];
         device_guard guard(sh.device);
-        auto &co = *r->co;
-        if (r->iter / co.slab_iters == co.slabs.size()) {
-            double *slab = nullptr;
-            HY_CUDA_CHECK(cudaMalloc(&slab, sizeof(double) * r->tc_doubles * co.slab_iters));
-            co.slabs.push_back(slab);
-        }
         // (The rows of the state variables come first in the batch's tc array; those of event equations are not recorded.)
-        HY_CUDA_CHECK(cudaMemcpyAsync(co.slabs[r->iter / co.slab_iters] + (r->iter % co.slab_iters) * r->tc_doubles, sh.d_tc,
-                                      sizeof(double) * r->tc_doubles, cudaMemcpyDeviceToDevice, sh.stream));
-        rec_push_times(sh, r);
-        ++r->iter;
+        HY_CUDA_CHECK(cudaMemcpyAsync(r->slot(), sh.d_tc, sizeof(double) * r->tc_doubles, cudaMemcpyDeviceToDevice,
+                                      sh.stream));
+        r->commit(sh);
         return HY_OK;
     } catch (...) {
         return translate_exception();
@@ -2714,8 +2663,7 @@ void hy_cout_rec_destroy(hy_cout_rec *r)
     delete r;
 }
 
-// make_c_out() (:1277-1317): forward[lane] != 0 for lanes integrated forwards in time (the padding row of the times is
-// +-inf by direction). *out = NULL if nothing was recorded. The recorder is destroyed either way.
+// The recorder is destroyed either way.
 int hy_cout_rec_finish(hy_batch *b, hy_cout_rec *rp, const unsigned char *forward, hy_cout **out)
 {
     std::unique_ptr<hy_cout_rec> r(rp);
@@ -2726,32 +2674,7 @@ int hy_cout_rec_finish(hy_batch *b, hy_cout_rec *rp, const unsigned char *forwar
         *out = nullptr;
         shard &sh = *b->shards[0];
         device_guard guard(sh.device);
-        const std::uint32_t n = sh.n;
-        const std::uint64_t iter = r->iter;
-        if (iter != 0u) {
-            auto &co = *r->co;
-            co.n_steps = iter;
-            const std::size_t rows = iter + 2u;
-            HY_CUDA_CHECK(cudaMalloc(&co.d_t_hi, sizeof(double) * rows * n));
-            HY_CUDA_CHECK(cudaMalloc(&co.d_t_lo, sizeof(double) * rows * n));
-            HY_CUDA_CHECK(cudaMalloc(&co.d_tm, sizeof(double) * n));
-            HY_CUDA_CHECK(cudaMalloc(&co.d_out, sizeof(double) * static_cast<std::size_t>(sh.n_eq) * n));
-            HY_CUDA_CHECK(cudaMemcpy2DAsync(co.d_t_hi, sizeof(double) * n, r->d_times, sizeof(double) * 2u * n,
-                                            sizeof(double) * n, iter + 1u, cudaMemcpyDeviceToDevice, sh.stream));
-            HY_CUDA_CHECK(cudaMemcpy2DAsync(co.d_t_lo, sizeof(double) * n, r->d_times + n, sizeof(double) * 2u * n,
-                                            sizeof(double) * n, iter + 1u, cudaMemcpyDeviceToDevice, sh.stream));
-            HY_CUDA_CHECK(cudaMalloc(&co.d_slabs, sizeof(double *) * co.slabs.size()));
-            HY_CUDA_CHECK(cudaMemcpyAsync(co.d_slabs, co.slabs.data(), sizeof(double *) * co.slabs.size(),
-                                          cudaMemcpyHostToDevice, sh.stream));
-            HY_CUDA_CHECK(cudaStreamSynchronize(sh.stream));
-            std::vector<double> pad(n), zero(n, 0.);
-            for (std::uint32_t i = 0; i < n; ++i) {
-                pad[i] = forward[i] != 0 ? std::numeric_limits<double>::infinity() : -std::numeric_limits<double>::infinity();
-            }
-            HY_CUDA_CHECK(cudaMemcpy(co.d_t_hi + (rows - 1u) * n, pad.data(), sizeof(double) * n, cudaMemcpyHostToDevice));
-            HY_CUDA_CHECK(cudaMemcpy(co.d_t_lo + (rows - 1u) * n, zero.data(), sizeof(double) * n, cudaMemcpyHostToDevice));
-            *out = r->co.release();
-        }
+        *out = r->finish(sh, forward);
         HY_CUDA_CHECK(cudaStreamSynchronize(sh.stream));
         return HY_OK;
     } catch (...) {
@@ -2773,12 +2696,12 @@ int hy_cout_eval(hy_cout *c, const double *tm, double *out)
             }
         }
         device_guard guard(c->device);
-        HY_CUDA_CHECK(cudaMemcpyAsync(c->d_tm, tm, sizeof(double) * c->n, cudaMemcpyHostToDevice, c->stream));
+        HY_CUDA_CHECK(cudaMemcpyAsync(c->d_tm.get(), tm, sizeof(double) * c->n, cudaMemcpyHostToDevice, c->stream));
         dev::k_cout_eval<<<(c->n + 127u) / 128u, 128, 0, c->stream>>>(
-            c->prog, c->n, static_cast<std::uint32_t>(c->n_steps + 2u), c->d_slabs, c->slab_iters, c->d_t_hi, c->d_t_lo,
-            c->d_tm, c->d_out);
+            c->prog, c->n, static_cast<std::uint32_t>(c->n_steps + 2u), c->d_slabs.get(), c->slab_iters,
+            c->d_t_hi.get(), c->d_t_lo.get(), c->d_tm.get(), c->d_out.get());
         HY_CUDA_CHECK(cudaGetLastError());
-        HY_CUDA_CHECK(cudaMemcpyAsync(out, c->d_out, sizeof(double) * static_cast<std::size_t>(c->n_eq) * c->n,
+        HY_CUDA_CHECK(cudaMemcpyAsync(out, c->d_out.get(), sizeof(double) * static_cast<std::size_t>(c->n_eq) * c->n,
                                       cudaMemcpyDeviceToHost, c->stream));
         HY_CUDA_CHECK(cudaStreamSynchronize(c->stream));
         return HY_OK;
@@ -2794,8 +2717,8 @@ int hy_cout_get_bounds(const hy_cout *c, double *lb, double *ub)
             throw std::invalid_argument("Null pointer passed to hy_cout_get_bounds()");
         }
         device_guard guard(c->device);
-        HY_CUDA_CHECK(cudaMemcpy(lb, c->d_t_hi, sizeof(double) * c->n, cudaMemcpyDeviceToHost));
-        HY_CUDA_CHECK(cudaMemcpy(ub, c->d_t_hi + c->n_steps * c->n, sizeof(double) * c->n, cudaMemcpyDeviceToHost));
+        HY_CUDA_CHECK(cudaMemcpy(lb, c->d_t_hi.get(), sizeof(double) * c->n, cudaMemcpyDeviceToHost));
+        HY_CUDA_CHECK(cudaMemcpy(ub, c->d_t_hi.get() + c->n_steps * c->n, sizeof(double) * c->n, cudaMemcpyDeviceToHost));
         return HY_OK;
     } catch (...) {
         return translate_exception();
@@ -2811,10 +2734,10 @@ int hy_cout_download(const hy_cout *c, double *times_hi, double *times_lo, doubl
         device_guard guard(c->device);
         const std::size_t n = c->n, rows = static_cast<std::size_t>(c->n_steps) + 2u;
         if (times_hi != nullptr) {
-            HY_CUDA_CHECK(cudaMemcpy(times_hi, c->d_t_hi, sizeof(double) * rows * n, cudaMemcpyDeviceToHost));
+            HY_CUDA_CHECK(cudaMemcpy(times_hi, c->d_t_hi.get(), sizeof(double) * rows * n, cudaMemcpyDeviceToHost));
         }
         if (times_lo != nullptr) {
-            HY_CUDA_CHECK(cudaMemcpy(times_lo, c->d_t_lo, sizeof(double) * rows * n, cudaMemcpyDeviceToHost));
+            HY_CUDA_CHECK(cudaMemcpy(times_lo, c->d_t_lo.get(), sizeof(double) * rows * n, cudaMemcpyDeviceToHost));
         }
         if (tcs != nullptr) {
             // One iteration = [n_eq][order + 1][batch] doubles; the slabs hold slab_iters iterations each, the last
@@ -2826,7 +2749,7 @@ int hy_cout_download(const hy_cout *c, double *times_hi, double *times_lo, doubl
                     break;
                 }
                 const std::size_t count = std::min<std::size_t>(c->slab_iters, c->n_steps - first);
-                HY_CUDA_CHECK(cudaMemcpy(tcs + first * it_doubles, c->slabs[s], sizeof(double) * count * it_doubles,
+                HY_CUDA_CHECK(cudaMemcpy(tcs + first * it_doubles, c->slabs[s].get(), sizeof(double) * count * it_doubles,
                                          cudaMemcpyDeviceToHost));
             }
         }

@@ -50,44 +50,42 @@ __global__ void k_d_output(program P, std::uint32_t n, const double *tc, const d
     }
 }
 
-// ---- propagate_grid() (src/taylor_adaptive_batch.cpp:1545-2055): per-lane bookkeeping and dense-output
-// sampling between the lock-step steps. One thread per lane. ----
-struct grid_state {
-    const double *grid; // [n_pts][batch]
-    std::uint32_t n_pts;
-    double *out;               // [n_pts][n_eq][batch], NaN-filled
-    const double *max_delta_t; // positive per-lane limits or nullptr (+inf)
-    std::uint32_t *cur_idx;    // first grid point not yet written, per lane
-    double *rem_hi, *rem_lo;   // remaining time to the last grid point (double-length)
-    unsigned char *t_dir;      // 1: forward
-    double *dt_limit;          // signed limit of the next step
-    unsigned *flags;           // [0] grid points left in some lane, [1] non-finite state, [2] overflow of rem
+// ---- The reference's lock-step loop (src/taylor_adaptive_batch.cpp:1372-1527, and :1696-2053 for propagate_grid()):
+// per-lane bookkeeping on the device between the steps. One thread per lane. ----
+struct lockstep_state {
+    const double *tf_hi, *tf_lo; // target times (tf_lo may be nullptr; a grid's target is its last row)
+    const double *max_delta_t;   // positive per-lane limits or nullptr (+inf)
+    double *rem_hi, *rem_lo;     // remaining time to the target (double-length)
+    unsigned char *t_dir;        // 1: forward
+    double *dt_limit;            // signed limit of the next step
+    unsigned *flags; // [0] number of lanes at their target in this iteration, [1] non-finite state, [2] overflow of rem
 };
 
-// After the initial propagate_until(grid[0]): remaining times, directions, counters (:1728-1760).
-__global__ void k_grid_init(batch D, grid_state G, double *min_h, double *max_h, unsigned long long *ts_count)
+// Before the first step: remaining times, directions, counters, limit of the first step (for a grid, :1728-1760).
+__global__ void k_lockstep_init(batch D, lockstep_state L, double *min_h, double *max_h, unsigned long long *ts_count)
 {
     const std::uint32_t lane = blockIdx.x * blockDim.x + threadIdx.x;
     if (lane >= D.n) {
         return;
     }
-    const dfl t{D.t_hi[lane], D.t_lo[lane]};
-    const dfl rem = dfl_sub(dfl{G.grid[static_cast<std::size_t>(G.n_pts - 1u) * D.n + lane], 0.}, t);
+    const dfl rem = dfl_sub(dfl{L.tf_hi[lane], L.tf_lo != nullptr ? L.tf_lo[lane] : 0.}, dfl{D.t_hi[lane], D.t_lo[lane]});
     if (!(isfinite(rem.hi) && isfinite(rem.lo))) {
-        atomicOr(G.flags + 2, 1u);
+        atomicOr(L.flags + 2, 1u);
     }
-    G.rem_hi[lane] = rem.hi;
-    G.rem_lo[lane] = rem.lo;
-    G.t_dir[lane] = dfl_ge0(rem) ? 1 : 0;
-    G.cur_idx[lane] = 1u;
+    L.rem_hi[lane] = rem.hi;
+    L.rem_lo[lane] = rem.lo;
+    const bool dir = dfl_ge0(rem);
+    L.t_dir[lane] = dir ? 1 : 0;
     min_h[lane] = CUDART_INF;
     max_h[lane] = 0.;
     ts_count[lane] = 0ull;
+    L.dt_limit[lane] = step_limit(dir, rem, L.max_delta_t != nullptr ? L.max_delta_t[lane] : CUDART_INF);
 }
 
-// After a step: counters, min/max |h|, remaining time, outcome (:1915-1971).
-__global__ void k_grid_book(batch D, grid_state G, long long *outcome, double *min_h, double *max_h,
-                            unsigned long long *ts_count)
+// After a lock-step step (:1402-1460, :1915-1971): counters, min/max |h|, remaining time, outcome, limit of the next
+// step.
+__global__ void k_lockstep_book(batch D, lockstep_state L, long long *outcome, double *min_h, double *max_h,
+                                unsigned long long *ts_count)
 {
     const std::uint32_t lane = blockIdx.x * blockDim.x + threadIdx.x;
     if (lane >= D.n) {
@@ -96,7 +94,7 @@ __global__ void k_grid_book(batch D, grid_state G, long long *outcome, double *m
     const long long oc = D.step_outcome[lane];
     const double h = D.last_h[lane];
     if (oc == HY_OUTCOME_ERR_NF_STATE) {
-        atomicOr(G.flags + 1, 1u);
+        atomicOr(L.flags + 1, 1u);
     } else {
         ts_count[lane] += (h != 0.) ? 1ull : 0ull;
         if (oc == HY_OUTCOME_SUCCESS) {
@@ -104,18 +102,29 @@ __global__ void k_grid_book(batch D, grid_state G, long long *outcome, double *m
             min_h[lane] = fmin(min_h[lane], ah);
             max_h[lane] = fmax(max_h[lane], ah);
         }
-        if (h == G.rem_hi[lane]) {
-            G.rem_hi[lane] = 0.;
-            G.rem_lo[lane] = 0.;
+        dfl rem{0., 0.};
+        if (h == L.rem_hi[lane]) {
+            atomicAdd(L.flags, 1u);
         } else {
-            const dfl rem = dfl_sub(dfl{G.grid[static_cast<std::size_t>(G.n_pts - 1u) * D.n + lane], 0.},
-                                    dfl{D.t_hi[lane], D.t_lo[lane]});
-            G.rem_hi[lane] = rem.hi;
-            G.rem_lo[lane] = rem.lo;
+            rem = dfl_sub(dfl{L.tf_hi[lane], L.tf_lo != nullptr ? L.tf_lo[lane] : 0.}, dfl{D.t_hi[lane], D.t_lo[lane]});
         }
+        L.rem_hi[lane] = rem.hi;
+        L.rem_lo[lane] = rem.lo;
+        L.dt_limit[lane]
+            = step_limit(L.t_dir[lane] != 0, rem, L.max_delta_t != nullptr ? L.max_delta_t[lane] : CUDART_INF);
     }
     outcome[lane] = oc;
 }
+
+// ---- propagate_grid() (src/taylor_adaptive_batch.cpp:1545-2055): dense-output sampling between the lock-step steps,
+// whose target is the last grid point. ----
+struct grid_state {
+    const double *grid; // [n_pts][batch]
+    std::uint32_t n_pts;
+    double *out;            // [n_pts][n_eq][batch], NaN-filled
+    std::uint32_t *cur_idx; // first grid point not yet written, per lane
+    unsigned *left;         // set when some lane has grid points left
+};
 
 // The grid points covered by the last step of a lane (:1811-1886): [first, last) from the lane's cursor, and the start
 // of the step (the Taylor coefficients are centred there).
@@ -123,13 +132,14 @@ struct grid_window {
     std::uint32_t first, last;
     dfl start;
 };
-__device__ __forceinline__ grid_window grid_covered(const batch &D, const grid_state &G, std::uint32_t lane)
+__device__ __forceinline__ grid_window grid_covered(const batch &D, const grid_state &G, const lockstep_state &L,
+                                                    std::uint32_t lane)
 {
     const std::size_t n = D.n;
     const dfl t{D.t_hi[lane], D.t_lo[lane]};
     const dfl cmp = dfl_sub(t, dfl{D.last_h[lane], 0.}); // start of the last step
     const dfl t0 = dfl_lt(cmp, t) ? cmp : t, t1 = dfl_lt(t, cmp) ? cmp : t;
-    const bool rem0 = G.rem_hi[lane] == 0. && G.rem_lo[lane] == 0.;
+    const bool rem0 = L.rem_hi[lane] == 0. && L.rem_lo[lane] == 0.;
     const std::uint32_t first = G.cur_idx[lane];
     std::uint32_t idx = first;
     while (idx < G.n_pts) {
@@ -147,14 +157,14 @@ __device__ __forceinline__ grid_window grid_covered(const batch &D, const grid_s
 // (a lane covers tens of grid points per step when the grid is dense: 36 x 21 coefficients x points per lane are too
 // much serial work for one thread). Reads the cursors only: k_grid_advance() moves them afterwards. Does nothing if a
 // non-finite state was detected in this iteration.
-__global__ void k_grid_sample(program P, batch D, grid_state G)
+__global__ void k_grid_sample(program P, batch D, grid_state G, lockstep_state L)
 {
     const std::uint32_t lane = blockIdx.x * blockDim.x + threadIdx.x, i = blockIdx.y;
-    if (lane >= D.n || G.flags[1] != 0u) {
+    if (lane >= D.n || L.flags[1] != 0u) {
         return;
     }
     const std::size_t n = D.n;
-    const grid_window w = grid_covered(D, G, lane);
+    const grid_window w = grid_covered(D, G, L, lane);
     const double *c = D.tc + static_cast<std::size_t>(i) * (P.order + 1u) * n + lane;
     for (std::uint32_t idx = w.first; idx < w.last; ++idx) {
         const dfl g{G.grid[static_cast<std::size_t>(idx) * n + lane], 0.};
@@ -164,85 +174,18 @@ __global__ void k_grid_sample(program P, batch D, grid_state G)
     }
 }
 
-// The cursors past the grid points k_grid_sample() has written, then the limit of the next step (:1899-1912).
-__global__ void k_grid_advance(batch D, grid_state G)
+// The cursors past the grid points k_grid_sample() has written (:1899-1912).
+__global__ void k_grid_advance(batch D, grid_state G, lockstep_state L)
 {
     const std::uint32_t lane = blockIdx.x * blockDim.x + threadIdx.x;
-    if (lane >= D.n || G.flags[1] != 0u) {
+    if (lane >= D.n || L.flags[1] != 0u) {
         return;
     }
-    const grid_window w = grid_covered(D, G, lane);
+    const grid_window w = grid_covered(D, G, L, lane);
     G.cur_idx[lane] = w.last;
     if (w.last < G.n_pts) {
-        atomicOr(G.flags, 1u);
+        atomicOr(G.left, 1u);
     }
-    const dfl rem{G.rem_hi[lane], G.rem_lo[lane]};
-    const double mdt = G.max_delta_t != nullptr ? G.max_delta_t[lane] : CUDART_INF;
-    G.dt_limit[lane] = step_limit(G.t_dir[lane] != 0, rem, mdt);
-}
-
-// ---- propagate_until() with continuous output: the reference's lock-step loop
-// (src/taylor_adaptive_batch.cpp:1372-1527), per-lane bookkeeping on the device. ----
-struct prop_state {
-    const double *tf_hi, *tf_lo; // final times (tf_lo may be nullptr)
-    const double *max_delta_t;   // positive per-lane limits or nullptr (+inf)
-    double *rem_hi, *rem_lo;
-    unsigned char *t_dir;
-    double *dt_limit;  // signed limit of the next step
-    unsigned *flags;   // [0] number of lanes done at this iteration, [1] non-finite state, [2] overflow of rem
-};
-
-__global__ void k_prop_init(batch D, prop_state G, double *min_h, double *max_h, unsigned long long *ts_count)
-{
-    const std::uint32_t lane = blockIdx.x * blockDim.x + threadIdx.x;
-    if (lane >= D.n) {
-        return;
-    }
-    const dfl rem = dfl_sub(dfl{G.tf_hi[lane], G.tf_lo != nullptr ? G.tf_lo[lane] : 0.}, dfl{D.t_hi[lane], D.t_lo[lane]});
-    if (!(isfinite(rem.hi) && isfinite(rem.lo))) {
-        atomicOr(G.flags + 2, 1u);
-    }
-    G.rem_hi[lane] = rem.hi;
-    G.rem_lo[lane] = rem.lo;
-    const bool dir = dfl_ge0(rem);
-    G.t_dir[lane] = dir ? 1 : 0;
-    min_h[lane] = CUDART_INF;
-    max_h[lane] = 0.;
-    ts_count[lane] = 0ull;
-    G.dt_limit[lane] = step_limit(dir, rem, G.max_delta_t != nullptr ? G.max_delta_t[lane] : CUDART_INF);
-}
-
-// After a lock-step step (:1402-1460): counters, min/max |h|, remaining time, outcome, limit of the next step.
-__global__ void k_prop_book(batch D, prop_state G, long long *outcome, double *min_h, double *max_h,
-                            unsigned long long *ts_count)
-{
-    const std::uint32_t lane = blockIdx.x * blockDim.x + threadIdx.x;
-    if (lane >= D.n) {
-        return;
-    }
-    const long long oc = D.step_outcome[lane];
-    const double h = D.last_h[lane];
-    if (oc == HY_OUTCOME_ERR_NF_STATE) {
-        atomicOr(G.flags + 1, 1u);
-    } else {
-        ts_count[lane] += (h != 0.) ? 1ull : 0ull;
-        if (oc == HY_OUTCOME_SUCCESS) {
-            const double ah = fabs(h);
-            min_h[lane] = fmin(min_h[lane], ah);
-            max_h[lane] = fmax(max_h[lane], ah);
-        }
-        dfl rem{0., 0.};
-        if (h == G.rem_hi[lane]) {
-            atomicAdd(G.flags, 1u);
-        } else {
-            rem = dfl_sub(dfl{G.tf_hi[lane], G.tf_lo != nullptr ? G.tf_lo[lane] : 0.}, dfl{D.t_hi[lane], D.t_lo[lane]});
-        }
-        G.rem_hi[lane] = rem.hi;
-        G.rem_lo[lane] = rem.lo;
-        G.dt_limit[lane]
-            = step_limit(G.t_dir[lane] != 0, rem, G.max_delta_t != nullptr ? G.max_delta_t[lane] : CUDART_INF);
-    }
-    outcome[lane] = oc;
 }
 
 // Evaluation of a continuous output (src/continuous_output.cpp:640-960): per lane, upper_bound of the time in the
