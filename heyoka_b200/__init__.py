@@ -17,7 +17,7 @@ from ._capi import lib, check, HyError  # noqa: F401
 
 __all__ = [
     "expression", "make_vars", "par", "time", "sin", "cos", "tanh", "exp", "log", "sigmoid", "relu", "relup", "sqrt", "square", "pow", "sum",
-    "prod", "diff", "var_args", "var_ode_sys", "model", "taylor_adaptive_batch", "t_event_batch", "nt_event_batch", "event_direction", "continuous_output_batch", "taylor_outcome", "Program", "Batch", "order_from_tol", "HyError",
+    "prod", "diff", "var_args", "var_ode_sys", "model", "callback", "taylor_adaptive_batch", "t_event_batch", "nt_event_batch", "event_direction", "continuous_output_batch", "taylor_outcome", "Program", "Batch", "order_from_tol", "HyError",
 ]
 
 
@@ -552,6 +552,12 @@ class Batch:
         m = None if max_delta_t is None else np.ascontiguousarray(max_delta_t, dtype=np.float64)
         check(lib.hy_batch_check_grid(self._h, _dptr(g), g.shape[0], _dptr(m)))
 
+    def set_angles(self, sv_idx):
+        """The state variables the propagate entry points reduce into [0, 2pi) after every step (hy_batch_set_angles());
+        an empty list clears it."""
+        idx = np.ascontiguousarray(sv_idx, dtype=np.uint32)
+        check(lib.hy_batch_set_angles(self._h, idx.ctypes.data_as(C.POINTER(C.c_uint32)), idx.size))
+
     def launch_count(self):
         n = C.c_uint64()
         check(lib.hy_batch_launch_count(self._h, C.byref(n)))
@@ -708,6 +714,8 @@ class taylor_adaptive_batch:
         self._step_res = None
         self._prop_res = None
         self._tc = None
+        # The names of the state variables, in state-row order (the angle reducer's pre_hook()).
+        self._sv_names = [repr(lhs) for lhs, _ in getattr(P, "_keep", [])]
 
     def _make_batch(self, P, batch_size, device):
         return Batch(P, batch_size, device)
@@ -1075,6 +1083,16 @@ class taylor_adaptive_batch:
                 self._prop_res = [(STEP_LIMIT,) + r[1:] for r in self._prop_res]
                 return finish()
 
+    def _device_angles(self, callback, grid=False):
+        """The state-row indices of an angle reducer passed as callback (checked before any step, like the reference's
+        pre_hook()) when the reduction can run on the device, else None. A wrapped reducer is an ordinary callback."""
+        if not isinstance(callback, _callback.angle_reducer):
+            return None
+        idx = callback.sv_indices(self)
+        if self._with_events or (grid and self._b.n_shards != 0):
+            return None
+        return idx if self._b.kernel_info()["tape"] in ("hbm", "smem", "global", "global-cta") else None
+
     def propagate_until(self, ts, max_steps=0, max_delta_t=None, write_tc=False, callback=None, c_output=False):
         n = self._batch_size
         if np.ndim(ts) == 0:
@@ -1096,6 +1114,15 @@ class taylor_adaptive_batch:
                 raise ValueError("Invalid number of max timesteps specified in a Taylor integrator in batch mode: the "
                                  "batch size is %d, but the number of specified timesteps is %d" % (n, md.size))
             max_delta_t = md
+        angles = self._device_angles(callback)
+        if angles is not None:
+            # The angle reducer on the device, inside the propagation loop.
+            self._b.set_angles(angles)
+            try:
+                return self.propagate_until(ts, max_steps=max_steps, max_delta_t=max_delta_t, write_tc=write_tc,
+                                            c_output=c_output)
+            finally:
+                self._b.set_angles([])
         if self._with_events or (callback is not None and not c_output):
             return self._propagate_until_host(th, np.zeros(n) if tl is None else tl, max_delta_t, max_steps, write_tc,
                                               callback, c_output)
@@ -1153,6 +1180,14 @@ class taylor_adaptive_batch:
                 raise ValueError("Invalid number of max timesteps specified in a Taylor integrator in batch mode: the "
                                  "batch size is %d, but the number of specified timesteps is %d" % (n, md.size))
             max_delta_t = np.ascontiguousarray(md)
+        angles = self._device_angles(callback, grid=True)
+        if angles is not None:
+            # The angle reducer on the device, inside the grid loop.
+            self._b.set_angles(angles)
+            try:
+                return self.propagate_grid(g.reshape(-1, n), max_steps=max_steps, max_delta_t=max_delta_t)
+            finally:
+                self._b.set_angles([])
         if self._with_events or callback is not None or self._b.n_shards != 0:
             # (Host loop: events and step callbacks are host code; a batch sharded over several devices samples its grid
             # through the dense output of its shards.)
@@ -1311,3 +1346,7 @@ def _dfloat_add(ahi, alo, bhi, blo):
     u, v = _eft_dekker(xh, yh + xl)
     u, v = _eft_dekker(u, v + yl)
     return u, v
+
+
+from . import callback  # noqa: E402
+from . import callback as _callback  # noqa: E402

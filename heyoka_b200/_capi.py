@@ -138,6 +138,8 @@ SIGNATURES = {
     "hy_batch_reset_cooldowns": (C.c_int, [_vp, C.c_int64]),
     "hy_batch_get_cooldowns": (C.c_int, [_vp, C.POINTER(C.c_uint8), _dp, _dp]),
     "hy_batch_set_cooldowns": (C.c_int, [_vp, C.POINTER(C.c_uint8), _dp, _dp]),
+    "hy_batch_set_angles": (C.c_int, [_vp, C.POINTER(C.c_uint32), C.c_uint32]),
+    "hy_reduce_angles": (C.c_int, [_dp, C.c_uint64]),
     "hy_batch_launch_count": (C.c_int, [_vp, C.POINTER(C.c_uint64)]),
     "hy_batch_set_launch_config": (C.c_int, [_vp, C.c_uint32, C.c_uint32]),
     "hy_batch_set_kernel": (C.c_int, [_vp, C.c_int, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32]),

@@ -18,7 +18,7 @@ OBJDIR = os.path.join(ROOT, "build", "obj")
 LIB = os.path.join(LIBDIR, "libheyoka_b200.so")
 
 HOST_SOURCES = ["expression.cpp", "decompose.cpp", "model.cpp", "lower.cpp", "smem_plan.cpp", "nb_plan.cpp", "nn_plan.cpp",
-                "capi_host.cpp", "taylor_adaptive_batch.cpp", "var_ode_sys.cpp"]
+                "capi_host.cpp", "taylor_adaptive_batch.cpp", "var_ode_sys.cpp", "callback.cpp"]
 CUDA_SOURCES = ["batch.cu", "nn_inst.cu", "nb1_inst.cu"]
 # The cooperative kernel is instantiated per (lanes per thread, max threads per CTA, mode) family, one
 # object each (built in parallel).
@@ -70,7 +70,10 @@ def build(force=False, verbose=True):
         if src.endswith(".cu"):
             cmd = [nvcc] + NVCC_ARCH + COMMON + CUDA_FLAGS + ["-c", path, "-o", obj]
         else:
-            cmd = [nvcc] + NVCC_ARCH + COMMON + ["-Xcompiler", "-fPIC,-Wall,-Wextra", "-c", path, "-o", obj]
+            # -ffp-contract=off: no FMA contraction on hosts whose baseline has FMA (aarch64), so that the host arithmetic
+            # shared with the kernels (angle_reduce.hpp) gives their bits.
+            cmd = [nvcc] + NVCC_ARCH + COMMON + ["-Xcompiler", "-fPIC,-Wall,-Wextra,-ffp-contract=off", "-c", path, "-o",
+                                                 obj]
         jobs.append((obj, path, cmd))
     inst = os.path.join(CSRC, "coop_inst.cu")
     for n_lanes, maxt, gen in COOP_FAMILIES:

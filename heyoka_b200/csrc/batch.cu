@@ -290,6 +290,13 @@ struct shard {
     double *d_prop_min_h = nullptr, *d_prop_max_h = nullptr;
     unsigned long long *d_prop_n_steps = nullptr, *d_prop_iters = nullptr;
     unsigned char *d_skip = nullptr; // per-lane mask of the masked zero-length step (propagate_finish())
+    // The angle reducer (hy_batch_set_angles()): per state variable, 1 = reduced into [0, 2pi) after every step of the
+    // propagate entry points; angles_on = the list is not empty. The device copy stays allocated once made, so that
+    // setting and clearing the list around every propagation costs no allocation.
+    std::vector<unsigned char> angles;
+    unsigned char *d_angles = nullptr;
+    bool angles_on = false;
+    const unsigned char *prop_angles() const;
 
     // Scratch.
     double *d_gscratch = nullptr, *d_cscratch = nullptr; // the selection's (kernel_sel::gscratch, cscratch)
@@ -377,7 +384,7 @@ void shard::free_all() noexcept
           static_cast<void *>(d_snapshot), static_cast<void *>(d_counter), static_cast<void *>(d_flags),
           static_cast<void *>(d_nb_pairs), static_cast<void *>(d_nb_roles), static_cast<void *>(d_nb_consts),
           static_cast<void *>(d_nb_fac), static_cast<void *>(d_nn_wimg), static_cast<void *>(d_nn_out),
-          static_cast<void *>(d_tmap)}) {
+          static_cast<void *>(d_tmap), static_cast<void *>(d_angles)}) {
         if (p != nullptr) {
             cudaFree(p);
         }
@@ -1188,6 +1195,21 @@ void shard::launch(bool prop, const dev::run_args &R)
     ++n_launches;
 }
 
+// The rows the propagate entry points reduce (run_args::angles), or null. The N-body and dense-network kernels have no
+// reduction (their programs hold no angles): a non-empty list is refused there.
+const unsigned char *shard::prop_angles() const
+{
+    if (!angles_on) {
+        return nullptr;
+    }
+    if (sel.family == kernel_sel::nb || sel.family == kernel_sel::nn) {
+        throw hy::detail::not_implemented_error("The angle reducer runs on the device only in the cooperative and the "
+                                                "HBM kernels, not in the N-body or dense-network kernel selected for "
+                                                "this batch");
+    }
+    return d_angles;
+}
+
 namespace
 {
 
@@ -1474,7 +1496,7 @@ struct prop_ctx {
 };
 
 void propagate_phase1(shard &sh, const double *d_tf_hi, const double *d_tf_lo, const double *d_mdt, uint64_t max_steps,
-                      int write_tc, prop_ctx &c)
+                      int write_tc, const unsigned char *angles, prop_ctx &c)
 {
     const std::size_t state_doubles = static_cast<std::size_t>(sh.n_eq) * sh.n;
     HY_CUDA_CHECK(cudaMemcpyAsync(sh.d_snapshot, sh.d_state, sizeof(double) * state_doubles, cudaMemcpyDeviceToDevice,
@@ -1494,6 +1516,7 @@ void propagate_phase1(shard &sh, const double *d_tf_hi, const double *d_tf_lo, c
     c.R.write_tc = write_tc;
     c.R.flags = sh.d_flags;
     c.R.counter = sh.d_counter;
+    c.R.angles = angles;
     sh.launch(true, c.R);
     HY_CUDA_CHECK(cudaMemcpyAsync(&c.fl, sh.d_flags, sizeof(c.fl), cudaMemcpyDeviceToHost, sh.stream));
     HY_CUDA_CHECK(cudaStreamSynchronize(sh.stream));
@@ -1518,6 +1541,8 @@ void propagate_replay(shard &sh, prop_ctx &c, unsigned long long cap)
 }
 
 // ex: the flags of the whole batch (any_nf from phase 1, any_limit and max_iter from the last launch).
+// (With the angle reducer there is nothing to reduce here: every lane takes at least the first iteration of the
+// kernel's loop, a zero-length step for a lane already at its final time, and that step reduces it.)
 void propagate_finish(shard &sh, const dev::run_flags &ex, int write_tc)
 {
     const std::uint32_t gb = (sh.n + 255u) / 256u;
@@ -1573,10 +1598,15 @@ void download_prop(shard &sh, const prop_host &h, std::size_t pitch, std::size_t
 // batch: on_device). With io, the shard's slice of the state and times is uploaded before and its results downloaded
 // after its own kernel: the state right away, last_h (and the outcomes, if the iteration limit was hit) once the global
 // exits are known. Returns the flags of the whole batch.
+// With reduce, the angle reducer of hy_batch_set_angles() runs after every step.
 dev::run_flags propagate(hy_batch *b, const double *tf_hi, const double *tf_lo, const double *mdt, int on_device,
-                         uint64_t max_steps, int write_tc, const prop_host *io)
+                         uint64_t max_steps, int write_tc, const prop_host *io, bool reduce = true)
 {
     std::vector<prop_ctx> ctx(b->shards.size());
+    std::vector<const unsigned char *> angles(b->shards.size());
+    for (std::size_t i = 0; i < b->shards.size(); ++i) {
+        angles[i] = reduce ? b->shards[i]->prop_angles() : nullptr;
+    }
     for_each_shard(b, [&](shard &sh, std::size_t i) {
         const std::size_t off = b->off[i];
         if (io != nullptr) {
@@ -1586,7 +1616,7 @@ dev::run_flags propagate(hy_batch *b, const double *tf_hi, const double *tf_lo, 
             rows_h2d(sh, sh.d_t_lo, io->t_lo_in, 1u, b->n, off);
         }
         propagate_phase1(sh, stage(sh, tf_hi, on_device, off, 0), stage(sh, tf_lo, on_device, off, 1),
-                         stage(sh, mdt, on_device, off, 2), max_steps, write_tc, ctx[i]);
+                         stage(sh, mdt, on_device, off, 2), max_steps, write_tc, angles[i], ctx[i]);
         if (io != nullptr) {
             download_prop(sh, *io, b->n, off); // (speculative: a non-finite lane anywhere makes every shard run again)
         }
@@ -1887,6 +1917,45 @@ int hy_batch_get_kernel(const hy_batch *b, hy_kernel_info *out)
     out->tmem_cols_per_warp = 0u; // (sm_90 has no tensor memory)
     out->reserved = 0u;
     return HY_OK;
+}
+
+int hy_batch_set_angles(hy_batch *b, const uint32_t *sv_idx, uint32_t n)
+{
+    try {
+        if (b == nullptr || (n != 0u && sv_idx == nullptr)) {
+            throw std::invalid_argument("Null pointer passed to hy_batch_set_angles()");
+        }
+        std::vector<unsigned char> mask(b->n_eq, 0u);
+        for (uint32_t k = 0; k < n; ++k) {
+            if (sv_idx[k] >= b->n_eq) {
+                throw std::invalid_argument("Invalid state variable index " + std::to_string(sv_idx[k])
+                                            + " passed to hy_batch_set_angles(): the system has "
+                                            + std::to_string(b->n_eq) + " state variables");
+            }
+            if (mask[sv_idx[k]] != 0u) {
+                throw std::invalid_argument("The state variable index " + std::to_string(sv_idx[k])
+                                            + " was passed twice to hy_batch_set_angles()");
+            }
+            mask[sv_idx[k]] = 1u;
+        }
+        for (auto &sh : b->shards) {
+            sh->angles_on = n != 0u;
+            if (n == 0u) {
+                continue;
+            }
+            device_guard guard(sh->device);
+            if (sh->d_angles == nullptr) {
+                sh->d_angles = sh->dalloc<unsigned char>(b->n_eq);
+            }
+            // (Ordered on the shard's stream after the launches that read the previous list.)
+            sh->angles = mask;
+            HY_CUDA_CHECK(cudaMemcpyAsync(sh->d_angles, sh->angles.data(), sh->angles.size(), cudaMemcpyHostToDevice,
+                                          sh->stream));
+        }
+        return HY_OK;
+    } catch (...) {
+        return translate_exception();
+    }
 }
 
 int hy_batch_upload(hy_batch *b, const double *state, const double *pars, const double *t_hi, const double *t_lo)
@@ -2235,6 +2304,7 @@ struct lockstep {
     dev_ptr<unsigned> d_flags; // [0, 3) those of dev::lockstep_state, [3] one more word for the caller
     dev::lockstep_state L{};
     unsigned flags[4] = {0u, 0u, 0u, 0u}; // as last read back
+    const unsigned char *angles = nullptr; // the rows every step reduces (shard::prop_angles()), or null
 
     // d_tf_hi, d_tf_lo: the target times on the device (d_tf_lo may be null); max_delta_t: host array or null.
     lockstep(shard &s, const double *d_tf_hi, const double *d_tf_lo, const double *max_delta_t)
@@ -2277,6 +2347,7 @@ struct lockstep {
         R.write_tc = 1;
         R.flags = sh.d_flags;
         R.counter = sh.d_counter;
+        R.angles = angles;
         sh.launch(false, R);
         HY_CUDA_CHECK(cudaMemsetAsync(d_flags.get(), 0, sizeof(flags), sh.stream));
         dev::k_lockstep_book<<<blocks(), 128, 0, sh.stream>>>(sh.view(), L, sh.d_prop_outcome, sh.d_prop_min_h,
@@ -2286,6 +2357,26 @@ struct lockstep {
     void read()
     {
         HY_CUDA_CHECK(cudaMemcpyAsync(flags, d_flags.get(), sizeof(flags), cudaMemcpyDeviceToHost, sh.stream));
+        HY_CUDA_CHECK(cudaStreamSynchronize(sh.stream));
+    }
+    // After an iteration in which a lane went non-finite: the reference returns before the step callback, so the
+    // reduction of that step is undone. The reduced rows are evaluated again from the step's Taylor coefficients with
+    // the step's h (the same polynomial evaluation as the step kernel's, so the same bits).
+    void undo_reduction()
+    {
+        if (angles == nullptr) {
+            return;
+        }
+        const std::uint32_t n = sh.n;
+        dev::k_d_output<<<(n + 127u) / 128u, 128, 0, sh.stream>>>(sh.prog, n, sh.d_tc, sh.d_last_h, sh.d_d_out);
+        HY_CUDA_CHECK(cudaGetLastError());
+        ++sh.n_launches;
+        for (std::uint32_t i = 0; i < sh.n_eq; ++i) {
+            if (sh.angles[i] != 0u) {
+                HY_CUDA_CHECK(cudaMemcpyAsync(sh.d_state + std::size_t(i) * n, sh.d_d_out + std::size_t(i) * n,
+                                              sizeof(double) * n, cudaMemcpyDeviceToDevice, sh.stream));
+            }
+        }
         HY_CUDA_CHECK(cudaStreamSynchronize(sh.stream));
     }
 };
@@ -2320,6 +2411,7 @@ int hy_batch_propagate_grid(hy_batch *b, const double *grid, uint64_t n_pts, con
         shard &sh = *b->shards[0];
         device_guard guard(sh.device);
         const std::uint32_t n = sh.n;
+        const unsigned char *angles = sh.prop_angles();
 
         const std::size_t n_out = static_cast<std::size_t>(n_pts) * sh.n_eq * n, state_doubles = std::size_t(sh.n_eq) * n;
         const auto d_grid = dev_alloc<double>(n_pts * n), d_out = dev_alloc<double>(n_out);
@@ -2327,6 +2419,7 @@ int hy_batch_propagate_grid(hy_batch *b, const double *grid, uint64_t n_pts, con
         HY_CUDA_CHECK(cudaMemcpyAsync(d_grid.get(), grid, sizeof(double) * n_pts * n, cudaMemcpyHostToDevice, sh.stream));
         // The target of every lane is its last grid point.
         lockstep ls(sh, d_grid.get() + (n_pts - 1u) * n, nullptr, max_delta_t);
+        ls.angles = angles;
         dev::k_fill_double<<<static_cast<unsigned>((n_out + 255u) / 256u), 256, 0, sh.stream>>>(
             d_out.get(), n_out, std::numeric_limits<double>::quiet_NaN());
         HY_CUDA_CHECK(cudaGetLastError());
@@ -2338,9 +2431,9 @@ int hy_batch_propagate_grid(hy_batch *b, const double *grid, uint64_t n_pts, con
         };
 
         // Up to the first grid point (a zero-length step when the time is already there: it brings the Taylor
-        // coefficients up to date), :1697-1706.
+        // coefficients up to date), :1697-1706. The reference calls no step callback there: no reduction.
         {
-            propagate(b, d_grid.get(), nullptr, ls.L.max_delta_t, 1, max_steps, 1, nullptr);
+            propagate(b, d_grid.get(), nullptr, ls.L.max_delta_t, 1, max_steps, 1, nullptr, false);
             std::vector<long long> oc(n);
             HY_CUDA_CHECK(cudaMemcpyAsync(oc.data(), sh.d_prop_outcome, sizeof(long long) * n, cudaMemcpyDeviceToHost,
                                           sh.stream));
@@ -2381,6 +2474,7 @@ int hy_batch_propagate_grid(hy_batch *b, const double *grid, uint64_t n_pts, con
             HY_CUDA_CHECK(cudaGetLastError());
             ls.read();
             if (ls.flags[1] != 0u) {
+                ls.undo_reduction();
                 break; // non-finite state: nothing further is written (:1973-1978)
             }
             if (++iter == max_steps) {
@@ -2552,6 +2646,7 @@ int hy_batch_propagate_until_cout_cb(hy_batch *b, const double *t_final_hi, cons
                                           sh.stream));
         }
         lockstep ls(sh, d_tf.get(), t_final_lo != nullptr ? d_tf.get() + n : nullptr, max_delta_t);
+        ls.angles = sh.prop_angles();
         hy_cout_rec rec(sh);
         // The step kernel writes the coefficients of every iteration straight into their slot of the recording; the
         // batch's own tc array is put back however the loop ends.
@@ -2575,6 +2670,7 @@ int hy_batch_propagate_until_cout_cb(hy_batch *b, const double *t_final_hi, cons
             ls.iterate();
             ls.read();
             if (ls.flags[1] != 0u) {
+                ls.undo_reduction();
                 break; // non-finite state: this iteration is not recorded (:1462-1467)
             }
             rec.commit(sh); // update_c_out(), :1320-1346

@@ -16,6 +16,7 @@
 #include <heyoka_b200/taylor_decompose.hpp>
 #include <heyoka_b200/var_ode_sys.hpp>
 
+#include "angle_reduce.hpp"
 #include "capi_common.hpp"
 #include "program.hpp"
 
@@ -398,6 +399,18 @@ int hy_model_ffnn(const hy_ex *const *inputs, uint32_t n_in, const uint32_t *nn_
     } catch (...) {
         return translate_exception();
     }
+}
+
+int hy_reduce_angles(double *x, uint64_t n)
+{
+    if (n != 0u && x == nullptr) {
+        hy::detail::set_last_error("Null pointer passed to hy_reduce_angles()");
+        return HY_ERR_INVALID_ARG;
+    }
+    for (uint64_t i = 0; i < n; ++i) {
+        x[i] = hy::detail::reduce_angle(x[i]);
+    }
+    return HY_OK;
 }
 
 int hy_order_from_tol(double tol, uint32_t *order)

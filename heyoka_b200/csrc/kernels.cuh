@@ -28,6 +28,7 @@
 #include <cuda_runtime.h>
 #include <math_constants.h>
 
+#include "angle_reduce.hpp"
 #include "device_program.cuh"
 #include "recurrences.cuh"
 #include "fused.cuh"
@@ -56,6 +57,9 @@ struct run_args {
     // step: lanes flagged here are left untouched (no state, time, outcome or tc write). Used for the zero-length
     // re-expansion of the lanes that finished a propagate_until() early (see batch.cu::propagate_finish()).
     const unsigned char *skip;
+    // The angle reducer (hy_batch_set_angles()): per state variable, 1 = the row is reduced into [0, 2pi) after every
+    // step, where finite. nullptr: no reduction. Only k_coop and k_hbm read it.
+    const unsigned char *angles;
 };
 
 // ================================================================================================
@@ -263,13 +267,17 @@ __device__ __forceinline__ double hbm_determine_h(const program &P, const hbm_ta
     return h_from_norms(P, m0, mp, mp1, max_delta_t);
 }
 
+// angles: the rows to reduce into [0, 2pi) (run_args::angles), or nullptr.
 __device__ __forceinline__ void hbm_update_state(const program &P, const hbm_tape &t, double h, double *state, double *tc,
-                                                 bool write)
+                                                 bool write, const unsigned char *angles)
 {
     const std::uint32_t pp1 = P.order + 1u;
     for (std::uint32_t i = 0; i < P.n_eq; ++i) {
         const auto r = t.row(i);
-        const double res = eval_poly(P, [&r](std::uint32_t o) { return r.at(o).v[0]; }, h);
+        double res = eval_poly(P, [&r](std::uint32_t o) { return r.at(o).v[0]; }, h);
+        if (angles != nullptr && __ldg(angles + i) != 0u) {
+            res = ::heyoka_b200::detail::reduce_angle(res);
+        }
         if (write) {
             state[static_cast<std::size_t>(i) * t.batch + t.lane] = res;
             if (tc != nullptr) {
@@ -380,7 +388,7 @@ __global__ void __launch_bounds__(256) k_hbm(program P, batch D, run_args R, dou
             tape.tm = t0.hi;
             hbm_jet(P, tape, D.state);
             const double h = hbm_determine_h(P, tape, mdt);
-            hbm_update_state(P, tape, h, D.state, R.write_tc ? D.tc : nullptr, valid);
+            hbm_update_state(P, tape, h, D.state, R.write_tc ? D.tc : nullptr, valid, R.angles);
             if (valid) {
                 const dfl nt = dfl_add(t0, dfl{h, 0.});
                 D.t_hi[lane] = nt.hi;
@@ -400,7 +408,11 @@ __global__ void __launch_bounds__(256) k_hbm(program P, batch D, run_args R, dou
                 tape.tm = lp.t.hi;
                 hbm_jet(P, tape, D.state);
                 const double h = hbm_determine_h(P, tape, cur_max);
-                hbm_update_state(P, tape, h, D.state, R.write_tc ? D.tc : nullptr, lp.running && valid);
+                // The replay of a propagation with a non-finite lane stops at the iteration where that lane went
+                // non-finite: the reference returns there before the step callback, so nothing is reduced.
+                const bool reduce = !(R.replay && lp.iter + 1u == R.iter_cap);
+                hbm_update_state(P, tape, h, D.state, R.write_tc ? D.tc : nullptr, lp.running && valid,
+                                 reduce ? R.angles : nullptr);
                 if (lp.running) {
                     lp.advance(h, cur_max, lane_state_nonfinite(P, D, lane), R, valid);
                 }
@@ -780,9 +792,11 @@ __device__ __forceinline__ double coop_determine_h(const program &P, const batch
 // State update of the warp's lanes: item = (state variable, lane); S.h holds the step sizes, S.running
 // which lanes may be written. Sets bit l of nf_mask if this thread produced a non-finite value for lane l.
 // A thread evaluates up to three polynomials side by side (their coefficients come from L2).
-template <int L, bool CTA = false>
+// ANG: the finite values of the rows flagged in `angles` (run_args::angles) are reduced into [0, 2pi).
+template <int L, bool CTA = false, bool ANG = false>
 __device__ __forceinline__ void coop_update_state(const program &P, const batch &D, const coop_smem<L> &S,
-                                                  const coef_view &cv, std::uint32_t lane0, unsigned &nf_mask)
+                                                  const coef_view &cv, std::uint32_t lane0, unsigned &nf_mask,
+                                                  const unsigned char *angles = nullptr)
 {
     constexpr int K = 3;
     const std::uint32_t tid = CTA ? threadIdx.x : (threadIdx.x & 31u), nthr = CTA ? blockDim.x : 32u;
@@ -808,9 +822,19 @@ __device__ __forceinline__ void coop_update_state(const program &P, const batch 
         for (int k = 0; k < K; ++k) {
             if (act[k] && lane_active) {
                 const std::uint32_t sv = (base + nthr * static_cast<std::uint32_t>(k)) / L;
-                D.state[static_cast<std::size_t>(sv) * n + glane] = res[k];
-                if (!isfinite(res[k])) {
-                    nf_mask |= 1u << l;
+                if constexpr (ANG) {
+                    double v = res[k];
+                    if (!isfinite(v)) {
+                        nf_mask |= 1u << l;
+                    } else if (angles[sv] != 0u) {
+                        v = ::heyoka_b200::detail::reduce_angle(v);
+                    }
+                    D.state[static_cast<std::size_t>(sv) * n + glane] = v;
+                } else {
+                    D.state[static_cast<std::size_t>(sv) * n + glane] = res[k];
+                    if (!isfinite(res[k])) {
+                        nf_mask |= 1u << l;
+                    }
                 }
             }
         }
@@ -891,7 +915,11 @@ __global__ void __launch_bounds__(MAXT, 1)
             }
             T::sync();
             unsigned nf_mask = 0u;
-            coop_update_state<L, CTA>(P, D, S, cv, lane0, nf_mask);
+            if (R.angles != nullptr) {
+                coop_update_state<L, CTA, true>(P, D, S, cv, lane0, nf_mask, R.angles);
+            } else {
+                coop_update_state<L, CTA>(P, D, S, cv, lane0, nf_mask);
+            }
             nf_mask = T::template reduce_or<L>(nf_mask);
             if (valid) {
                 const dfl nt = dfl_add(t0, dfl{h, 0.});
@@ -908,6 +936,8 @@ __global__ void __launch_bounds__(MAXT, 1)
             if (owner) {
                 lp.init(D, R, lane);
             }
+            // Iterations of the team's loop, the current one included (every running lane takes a step in each).
+            unsigned long long it = 0;
             while (T::any(owner && lp.running)) {
                 double cur_max = 0.;
                 if (owner) {
@@ -923,7 +953,13 @@ __global__ void __launch_bounds__(MAXT, 1)
                 }
                 T::sync();
                 unsigned nf_mask = 0u;
-                coop_update_state<L, CTA>(P, D, S, cv, lane0, nf_mask);
+                // (No reduction in the last iteration of a replay: see k_hbm.)
+                ++it;
+                if (R.angles != nullptr && !(R.replay && it == R.iter_cap)) {
+                    coop_update_state<L, CTA, true>(P, D, S, cv, lane0, nf_mask, R.angles);
+                } else {
+                    coop_update_state<L, CTA>(P, D, S, cv, lane0, nf_mask);
+                }
                 nf_mask = T::template reduce_or<L>(nf_mask);
                 if (owner && lp.running) {
                     lp.advance(h, cur_max, ((nf_mask >> tid) & 1u) != 0u, R, valid);

@@ -3,6 +3,8 @@
 // dense output :2251-2327, getters), include/heyoka/detail/dfloat.hpp.
 #include <heyoka_b200/taylor.hpp>
 
+#include <heyoka_b200/callback.hpp>
+
 #include <algorithm>
 #include <cmath>
 #include <cstdio>
@@ -84,6 +86,29 @@ inline void check(int st)
     if (st != HY_OK) {
         throw_from_status(st);
     }
+}
+
+// The angle list of hy_batch_set_angles() for the duration of one propagation.
+struct angle_scope {
+    hy_batch *b;
+    angle_scope(hy_batch *batch, const std::vector<std::uint32_t> &idx) : b(batch)
+    {
+        check(hy_batch_set_angles(b, idx.data(), static_cast<std::uint32_t>(idx.size())));
+    }
+    angle_scope(const angle_scope &) = delete;
+    angle_scope &operator=(const angle_scope &) = delete;
+    ~angle_scope()
+    {
+        hy_batch_set_angles(b, nullptr, 0u);
+    }
+};
+
+// The kernels that run the angle reducer on the device: every one but the N-body and dense-network kernels.
+bool device_reduces(const hy_batch *b)
+{
+    hy_kernel_info k{};
+    check(hy_batch_get_kernel(b, &k));
+    return k.tape_mode < 6;
 }
 
 } // namespace
@@ -1273,6 +1298,18 @@ taylor_adaptive_batch<double>::propagate_grid_impl(const std::vector<double> &gr
                                     + std::to_string(n) + ", but the number of specified timesteps is "
                                     + std::to_string(o.max_delta_t.size()));
     }
+    if (const auto *ar = o.cb ? o.cb.target<callback::angle_reducer>() : nullptr) {
+        const auto idx = ar->get_sv_indices(*this); // (the reference's pre_hook(): before any step)
+        if (!with_events() && m.devices.empty() && device_reduces(m.batch)) {
+            // The angle reducer on the device, inside the grid loop.
+            const angle_scope scope(m.batch, idx);
+            auto cb = std::move(o.cb);
+            o.cb = nullptr;
+            auto res = propagate_grid_impl(grid, std::move(o));
+            std::get<0>(res) = std::move(cb);
+            return res;
+        }
+    }
     if (o.cb || with_events() || !m.devices.empty()) {
         // A step callback (or events, whose callbacks also run on the host) after every step: the reference's loop on the
         // host, one device step per iteration. A batch sharded over several devices takes it too (the grid is sampled
@@ -1485,6 +1522,19 @@ taylor_adaptive_batch<double>::propagate_until_impl(const std::vector<double> &h
         }
     }
     const double *mdt = o.max_delta_t.empty() ? nullptr : o.max_delta_t.data();
+
+    if (const auto *ar = o.cb ? o.cb.target<callback::angle_reducer>() : nullptr) {
+        const auto idx = ar->get_sv_indices(*this); // (the reference's pre_hook(): before any step)
+        if (!with_events() && device_reduces(m.batch)) {
+            // The angle reducer on the device, inside the propagation loop: the paths without a step callback below.
+            const angle_scope scope(m.batch, idx);
+            auto cb = std::move(o.cb);
+            o.cb = nullptr;
+            auto res = propagate_until_impl(hi, lo, std::move(o));
+            std::get<1>(res) = std::move(cb);
+            return res;
+        }
+    }
 
     if (o.c_output && !with_events()) {
         // The reference's lock-step loop with the recording of the Taylor coefficients, on the device

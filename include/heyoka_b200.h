@@ -394,6 +394,17 @@ int hy_batch_get_cooldowns(hy_batch *, uint8_t *active, double *spent, double *c
  * m_te_cooldowns, src/detail/event_detection.cpp:1622-1645). */
 int hy_batch_set_cooldowns(hy_batch *, const uint8_t *active, const double *spent, const double *cooldown);
 
+/* The angle reducer (callback::angle_reducer, include/heyoka_b200/callback.hpp). hy_batch_set_angles() sets the state
+ * variables (indices into the state rows) that the propagate entry points reduce into [0, 2pi) after every step, on
+ * the device, where their values are finite: hy_batch_propagate_until{,_host,_dev}(), hy_batch_propagate_grid() (not
+ * its initial propagation to the first grid point) and hy_batch_propagate_until_cout{,_cb}(). hy_batch_step() never
+ * reduces. n = 0 clears the list; an index out of range or repeated: HY_ERR_INVALID_ARG. The list applies to every
+ * shard. With the N-body or dense-network kernel selected (tape_mode 6 to 9), the propagate entry points refuse a
+ * non-empty list with HY_ERR_NOT_IMPLEMENTED.
+ * hy_reduce_angles() applies the same reduction to n host values in place, with the same bits. */
+int hy_batch_set_angles(hy_batch *, const uint32_t *sv_idx, uint32_t n);
+int hy_reduce_angles(double *x, uint64_t n);
+
 /* Kernel launch statistics since creation (bench.py's gpu_launches). */
 int hy_batch_launch_count(const hy_batch *, uint64_t *n_launches);
 /* Name + average duration bookkeeping is done by the caller with CUDA events on the batch's stream. */

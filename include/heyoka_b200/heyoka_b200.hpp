@@ -4,6 +4,7 @@
 #ifndef HEYOKA_B200_HEYOKA_B200_HPP
 #define HEYOKA_B200_HEYOKA_B200_HPP
 
+#include <heyoka_b200/callback.hpp>
 #include <heyoka_b200/expression.hpp>
 #include <heyoka_b200/kw.hpp>
 #include <heyoka_b200/model.hpp>
