@@ -403,12 +403,14 @@ class Batch:
         s, p, th, tl = f(state), f(pars), f(t_hi), f(t_lo)
         check(lib.hy_batch_upload(self._h, _dptr(s), _dptr(p), _dptr(th), _dptr(tl)))
 
-    def download(self):
+    def download(self, state=True, times=True, last_h=True):
+        """(state, t_hi, t_lo, last_h); the arrays not asked for are None and are not copied."""
         P = self.program
-        state = np.empty((P.n_eq, self.n))
-        t_hi, t_lo, last_h = np.empty(self.n), np.empty(self.n), np.empty(self.n)
-        check(lib.hy_batch_download(self._h, _dptr(state), _dptr(t_hi), _dptr(t_lo), _dptr(last_h)))
-        return state, t_hi, t_lo, last_h
+        st = np.empty((P.n_eq, self.n)) if state else None
+        t_hi, t_lo = (np.empty(self.n), np.empty(self.n)) if times else (None, None)
+        lh = np.empty(self.n) if last_h else None
+        check(lib.hy_batch_download(self._h, _dptr(st), _dptr(t_hi), _dptr(t_lo), _dptr(lh)))
+        return st, t_hi, t_lo, lh
 
     def step_res(self):
         oc, h = np.empty(self.n, dtype=np.int64), np.empty(self.n)
@@ -497,6 +499,52 @@ class Batch:
         check(lib.hy_batch_propagate_grid(self._h, _dptr(grid), n_pts, None if md is None else _dptr(md),
                                           int(max_steps), _dptr(out)))
         return out
+
+    @staticmethod
+    def _event_callback(on_events, err):
+        """The hy_event_callback of the event propagations: on_events(evs, t_hi, t_lo, cont) gets the records as
+        events() gives them, their absolute times and the decision bytes; what it raises ends the propagation and is
+        kept in err."""
+        def tramp(_user, recs, t_hi, t_lo, n, cont):
+            try:
+                evs = [(r.lane, r.idx, bool(r.terminal), r.d_sgn, r.t, r.abs_der) for r in recs[:n]]
+                on_events(evs, t_hi, t_lo, cont)
+                return 1
+            except BaseException as e:  # noqa: BLE001 - carried across the C frame, re-raised by the caller
+                err.append(e)
+                return -1
+        return _capi.hy_event_callback(tramp)
+
+    def propagate_until_ev(self, t_hi, t_lo, max_delta_t, max_steps, on_events, c_output=False):
+        """hy_batch_propagate_until_ev(): propagate_until() of a batch with events on the device, on_events called for
+        the iterations that have event records (see _event_callback). Returns (continuous output or None, the
+        exception on_events raised or None)."""
+        f = lambda a: None if a is None else np.ascontiguousarray(np.broadcast_to(a, (self.n,)), dtype=np.float64)  # noqa
+        th, tl, md = f(t_hi), f(t_lo), f(max_delta_t)
+        err = []
+        tramp = self._event_callback(on_events, err)
+        h = C.c_void_p()
+        st = lib.hy_batch_propagate_until_ev(self._h, _dptr(th), _dptr(tl), _dptr(md), int(max_steps),
+                                             C.cast(tramp, C.c_void_p), None, C.byref(h) if c_output else None)
+        if st != _capi.HY_ERR_CALLBACK or not err:
+            check(st)
+        c_out = continuous_output_batch(h, self.program.n_eq, self.n, self.program.order) if h.value else None
+        return c_out, (err[0] if err else None)
+
+    def propagate_grid_ev(self, grid, max_delta_t, max_steps, on_events):
+        """hy_batch_propagate_grid_ev(): propagate_grid() of a batch with events on the device. Returns (the states at
+        the grid points [n_pts, n_eq, batch], the exception on_events raised or None)."""
+        grid = np.ascontiguousarray(grid, dtype=np.float64)
+        n_pts = grid.size // self.n
+        md = None if max_delta_t is None else np.ascontiguousarray(max_delta_t, dtype=np.float64)
+        out = np.empty((n_pts, self.program.n_eq, self.n))
+        err = []
+        tramp = self._event_callback(on_events, err)
+        st = lib.hy_batch_propagate_grid_ev(self._h, _dptr(grid), n_pts, _dptr(md), int(max_steps),
+                                            C.cast(tramp, C.c_void_p), None, _dptr(out))
+        if st != _capi.HY_ERR_CALLBACK or not err:
+            check(st)
+        return out, (err[0] if err else None)
 
     def d_output(self, tau):
         P = self.program
@@ -745,6 +793,8 @@ class taylor_adaptive_batch:
 
     @property
     def pars(self):
+        if self.__dict__.get("_pars_touched") is False:
+            self.__dict__["_pars_touched"] = True  # (inside the callbacks of a device event propagation)
         return self._pars
 
     @property
@@ -924,29 +974,47 @@ class taylor_adaptive_batch:
         if not evs:
             return
         t_copy = (self._t_hi.copy(), self._t_lo.copy())
+
+        def nt_time(m):
+            # new_time - last_h + t in double-length arithmetic (:889).
+            lane = evs[m][0]
+            hi, lo = _dfloat_add(t_copy[0][lane], t_copy[1][lane], -self._last_h[lane], 0.0)
+            hi, lo = _dfloat_add(hi, lo, evs[m][4], 0.0)
+            return float(hi)
+
+        def decide(m, ret):
+            lane, idx = evs[m][0], evs[m][1]
+            self._step_res[lane] = (idx if ret else -idx - 1, self._step_res[lane][1])
+        self._raise_event_excs(self._call_event_callbacks(evs, nt_time, decide))
+        self._check_time_kept(t_copy)
+
+    def _call_event_callbacks(self, evs, nt_time, decide):
+        """The callbacks of one step's events, evs as Batch.events() lists them: per lane, the non-terminal events, then
+        the terminal one. nt_time(m) is the absolute time of record m; decide(m, ret) takes the decision of the terminal
+        event m whose callback returned (ret True: continue). Returns the exceptions raised, as (lane, exception): a
+        lane stops at its first one, the other lanes go on."""
         excs = []
-        lanes = sorted({e[0] for e in evs})
-        for lane in lanes:
-            mine = [e for e in evs if e[0] == lane]
-            h = self._last_h[lane]
+        k = 0
+        while k < len(evs):
+            lane = evs[k][0]
+            j = k
+            while j < len(evs) and evs[j][0] == lane:
+                j += 1
             thrown = False
-            for (_, idx, terminal, d_sgn, t, _ad) in mine:
+            for m in range(k, j):
+                _, idx, terminal, d_sgn, _t, _ad = evs[m]
                 if terminal:
                     continue
-                # new_time - last_h + t in double-length arithmetic (:889).
-                hi, lo = _dfloat_add(t_copy[0][lane], t_copy[1][lane], -h, 0.0)
-                hi, lo = _dfloat_add(hi, lo, t, 0.0)
                 try:
-                    self._ntes[idx].callback(self, float(hi), d_sgn, lane)
+                    self._ntes[idx].callback(self, nt_time(m), d_sgn, lane)
                 except Exception as e:  # noqa: BLE001 - collected and re-raised below like the reference
                     excs.append((lane, e))
                     thrown = True
                     break
-            if thrown:
-                continue
-            te = [e for e in mine if e[2]]
-            if te:
-                _, idx, _, d_sgn, _t, _ad = te[0]
+            te = [m for m in range(k, j) if evs[m][2]]
+            if te and not thrown:
+                m = te[0]
+                _, idx, _, d_sgn, _t, _ad = evs[m]
                 ret = False
                 cb = self._tes[idx].callback
                 if cb is not None:
@@ -954,8 +1022,14 @@ class taylor_adaptive_batch:
                         ret = bool(cb(self, d_sgn, lane))
                     except Exception as e:  # noqa: BLE001
                         excs.append((lane, e))
-                        continue
-                self._step_res[lane] = (idx if ret else -idx - 1, self._step_res[lane][1])
+                        ret = None
+                if ret is not None:
+                    decide(m, ret)
+            k = j
+        return excs
+
+    @staticmethod
+    def _raise_event_excs(excs):
         if len(excs) == 1:
             raise excs[0][1]
         if excs:
@@ -964,11 +1038,111 @@ class taylor_adaptive_batch:
                 msg += "Batch index #%d:\n    Exception type: %s\n    Exception message: %s\n\n" % (
                     lane, type(e).__name__, e)
             raise RuntimeError(msg)
+
+    def _check_time_kept(self, t_copy):
         same = lambda a, b: np.array_equal(a, b, equal_nan=True)  # noqa: E731
         if not (same(self._t_hi, t_copy[0]) and same(self._t_lo, t_copy[1])):
             i = int(np.argmax(~((self._t_hi == t_copy[0]) | (np.isnan(self._t_hi) & np.isnan(t_copy[0])))))
             raise RuntimeError("The invocation of one or more event callbacks resulted in the alteration of the time "
                                "coordinate of the integrator at the batch index %d - this is not supported" % i)
+
+    # --- events on the device (hy_batch_propagate_until_ev() / hy_batch_propagate_grid_ev()) ---------------------------
+    # The device loop calls back to the host only in the iterations that have event records. While the callbacks of
+    # such an iteration run, the mirrors are fetched from the device on first access (_LAZY); afterwards the state and
+    # parameters a callback could have written go back up, as the host loop's next _push() would send them.
+    def _device_events(self, callback):
+        """Whether a propagation runs its event loop on the device: events and no step callback. (A batch substituted
+        for the device one, such as the tests' CPU oracle, runs the host loop.)"""
+        return self._with_events and callback is None and isinstance(self._b, Batch)
+
+    def _device_event_callbacks(self, evs, t_hi, t_lo, cont):
+        d = self.__dict__
+        d["_stale"] = set(_LAZY)
+        d["_pars_touched"] = False
+        d["_t_seen"] = None
+        d["_ev_decisions"] = []
+        try:
+            def decide(m, ret):
+                cont[m] = 1 if ret else 0
+                lane, idx = evs[m][0], evs[m][1]
+                d["_ev_decisions"].append((lane, idx if ret else -idx - 1))
+                if "_step_res" not in d["_stale"]:
+                    d["_step_res"][lane] = (d["_ev_decisions"][-1][1], d["_step_res"][lane][1])
+            self._raise_event_excs(self._call_event_callbacks(evs, lambda m: float(t_hi[m]), decide))
+            if d["_t_seen"] is not None:
+                self._check_time_kept(d["_t_seen"])
+        finally:
+            st = None if "_state" in d["_stale"] else d["_state"]
+            pr = self._pars if d["_pars_touched"] and self._prog.n_pars else None
+            if st is not None or pr is not None:
+                self._b.upload(st, pr)
+            d["_pars_touched"] = None
+
+    def _fetch(self, name):
+        d, b = self.__dict__, self._b
+        if name == "_state":
+            d["_state"] = b.download(times=False, last_h=False)[0]
+        elif name in ("_t_hi", "_t_lo"):
+            _, d["_t_hi"], d["_t_lo"], _ = b.download(state=False, last_h=False)
+            d["_t_seen"] = (d["_t_hi"].copy(), d["_t_lo"].copy())
+            d["_stale"].discard("_t_hi" if name == "_t_lo" else "_t_lo")
+        elif name == "_last_h":
+            d["_last_h"] = b.download(state=False, times=False)[3]
+        elif name == "_tc":
+            d["_tc"] = b.tc()
+        elif name == "_step_res":
+            oc, h = b.step_res()
+            d["_step_res"] = list(zip(oc.tolist(), h.tolist()))
+            for lane, outcome in d.get("_ev_decisions", ()):  # (taken in this iteration, not yet on the device)
+                d["_step_res"][lane] = (outcome, d["_step_res"][lane][1])
+        else:
+            oc, mn, mx, ns = b.prop_res()
+            d["_prop_res"] = list(zip(oc.tolist(), mn.tolist(), mx.tolist(), ns.tolist()))
+        d["_stale"].discard(name)
+
+    def _end_device_call(self, err):
+        """After an event propagation on the device: the mirrors from the device in one go, or, if a callback raised,
+        those the last callbacks did not fetch (the others keep what the callbacks left in them, as in the host
+        loop), then the exception."""
+        d = self.__dict__
+        if err is None:
+            d["_stale"] = set()
+            self._pull(True)
+            oc, h = self._b.step_res()
+            self._step_res = list(zip(oc.tolist(), h.tolist()))
+            oc, mn, mx, ns = self._b.prop_res()
+            self._prop_res = list(zip(oc.tolist(), mn.tolist(), mx.tolist(), ns.tolist()))
+            return
+        for name in _LAZY:
+            if name in d["_stale"]:
+                self._fetch(name)
+        d["_stale"] = set()
+        raise err
+
+    def _device_event_call(self, run):
+        self._push()
+        cls = self.__class__
+        self.__class__ = _lazy_class(cls)
+        try:
+            res, err = run()
+        except BaseException:
+            self.__dict__["_stale"] = set()
+            self.__class__ = cls
+            raise
+        try:
+            self._end_device_call(err)
+        finally:
+            self.__class__ = cls
+            self.__dict__["_ev_decisions"] = []
+        return res
+
+    def _propagate_until_events(self, th, tl, max_delta_t, max_steps, c_output):
+        return self._device_event_call(lambda: self._b.propagate_until_ev(
+            th, tl, max_delta_t, max_steps, self._device_event_callbacks, c_output))
+
+    def _propagate_grid_events(self, grid, max_delta_t, max_steps):
+        return self._device_event_call(lambda: self._b.propagate_grid_ev(
+            grid, max_delta_t, max_steps, self._device_event_callbacks))
 
     def step(self, max_delta_ts=None, write_tc=False):
         if max_delta_ts is not None:
@@ -1006,6 +1180,8 @@ class taylor_adaptive_batch:
         if not (np.all(np.isfinite(rem_hi)) and np.all(np.isfinite(rem_lo))):
             raise OverflowError("The final time passed to the propagate_until() function of an adaptive Taylor "
                                 "integrator in batch mode results in an overflow condition")
+        if self._device_events(callback):
+            return self._propagate_until_events(th, tl, max_delta_t, max_steps, c_output)
         t_dir = (rem_hi > 0) | ((rem_hi == 0) & (rem_lo >= 0))
         self._prop_res = [(0, 0.0, 0.0, 0)] * n
         # Continuous output (integrators with events): the iterations of this loop are recorded on the device
@@ -1188,6 +1364,8 @@ class taylor_adaptive_batch:
                 return self.propagate_grid(g.reshape(-1, n), max_steps=max_steps, max_delta_t=max_delta_t)
             finally:
                 self._b.set_angles([])
+        if self._device_events(callback) and self._b.n_shards == 0:
+            return self._propagate_grid_events(g.reshape(-1, n), max_delta_t, max_steps)
         if self._with_events or callback is not None or self._b.n_shards != 0:
             # (Host loop: events and step callbacks are host code; a batch sharded over several devices samples its grid
             # through the dense output of its shards.)
@@ -1310,6 +1488,38 @@ class taylor_adaptive_batch:
             hi, lo = _dfloat_add(self._t_hi, self._t_lo, -self._last_h, np.zeros(n))
             tau, _ = _dfloat_add(t, np.zeros(n), -hi, -lo)
         return self._b.d_output(tau)
+
+
+# The mirrors a device event propagation fetches on first access while callbacks run (taylor_adaptive_batch._fetch()).
+_LAZY = ("_state", "_t_hi", "_t_lo", "_last_h", "_tc", "_step_res", "_prop_res")
+
+
+def _lazy_mirror(name):
+    def get(self):
+        if name in self.__dict__.get("_stale", ()):
+            self._fetch(name)
+        return self.__dict__.get(name)
+
+    def put(self, v):
+        stale = self.__dict__.get("_stale", ())
+        if name in stale:
+            if name in ("_t_hi", "_t_lo"):
+                self._fetch(name)  # (the times as they were, for the check that callbacks keep them)
+            stale.discard(name)
+        self.__dict__[name] = v
+    return property(get, put)
+
+
+_LAZY_CLASSES = {}
+
+
+def _lazy_class(cls):
+    """cls with the mirrors of _LAZY fetched on first access: an integrator takes it only for the duration of a device
+    event propagation, so that the host loops' per-lane accesses stay plain attribute reads."""
+    c = _LAZY_CLASSES.get(cls)
+    if c is None:
+        c = _LAZY_CLASSES[cls] = type(cls.__name__, (cls,), {n: _lazy_mirror(n) for n in _LAZY})
+    return c
 
 
 def _var_initial_state(vsys, state, batch):

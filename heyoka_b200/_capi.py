@@ -65,6 +65,10 @@ _dp = C.POINTER(C.c_double)
 _vp = C.c_void_p
 _vpp = C.POINTER(C.c_void_p)
 
+# hy_event_callback: (user, recs, t_hi, t_lo, n_rec, cont) -> int.
+hy_event_callback = C.CFUNCTYPE(C.c_int, C.c_void_p, C.POINTER(hy_event_rec), _dp, _dp, C.c_uint32,
+                                C.POINTER(C.c_uint8))
+
 # name -> (restype, argtypes); mirrors include/heyoka_b200.h one to one.
 SIGNATURES = {
     "hy_last_error": (C.c_char_p, []),
@@ -138,6 +142,8 @@ SIGNATURES = {
     "hy_batch_reset_cooldowns": (C.c_int, [_vp, C.c_int64]),
     "hy_batch_get_cooldowns": (C.c_int, [_vp, C.POINTER(C.c_uint8), _dp, _dp]),
     "hy_batch_set_cooldowns": (C.c_int, [_vp, C.POINTER(C.c_uint8), _dp, _dp]),
+    "hy_batch_propagate_until_ev": (C.c_int, [_vp, _dp, _dp, _dp, C.c_uint64, C.c_void_p, C.c_void_p, _vpp]),
+    "hy_batch_propagate_grid_ev": (C.c_int, [_vp, _dp, C.c_uint64, _dp, C.c_uint64, C.c_void_p, C.c_void_p, _dp]),
     "hy_batch_set_angles": (C.c_int, [_vp, C.POINTER(C.c_uint32), C.c_uint32]),
     "hy_reduce_angles": (C.c_int, [_dp, C.c_uint64]),
     "hy_batch_launch_count": (C.c_int, [_vp, C.POINTER(C.c_uint64)]),

@@ -8,6 +8,7 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <functional>
 #include <initializer_list>
 #include <limits>
 #include <memory>
@@ -2349,6 +2350,11 @@ struct lockstep {
         R.counter = sh.d_counter;
         R.angles = angles;
         sh.launch(false, R);
+        book();
+    }
+    // The bookkeeping of the step just taken (an event step runs shard::ev_step(L.dt_limit, 0) and its callbacks first).
+    void book()
+    {
         HY_CUDA_CHECK(cudaMemsetAsync(d_flags.get(), 0, sizeof(flags), sh.stream));
         dev::k_lockstep_book<<<blocks(), 128, 0, sh.stream>>>(sh.view(), L, sh.d_prop_outcome, sh.d_prop_min_h,
                                                                 sh.d_prop_max_h, sh.d_prop_n_steps);
@@ -2773,6 +2779,361 @@ int hy_cout_rec_finish(hy_batch *b, hy_cout_rec *rp, const unsigned char *forwar
         *out = r->finish(sh, forward);
         HY_CUDA_CHECK(cudaStreamSynchronize(sh.stream));
         return HY_OK;
+    } catch (...) {
+        return translate_exception();
+    }
+}
+
+// ------------------------------------------------------------------------------------------------
+// Propagation of a batch with event equations (hy_batch_propagate_until_ev(), hy_batch_propagate_grid_ev()): the
+// reference's lock-step loop (src/taylor_adaptive_batch.cpp:1372-1527, :1696-2053) over event steps, with the
+// bookkeeping on the device. The host takes part in an iteration only when some lane produced an event record: it
+// receives the records with their absolute times and hands back the terminal-event decisions.
+// ------------------------------------------------------------------------------------------------
+namespace
+{
+
+struct ev_shard {
+    std::unique_ptr<lockstep> ls;
+    dev_ptr<double> d_tf;          // target times of propagate_until() (hi, lo)
+    std::vector<hy_event_rec> recs; // live records of the iteration, lanes local to the shard
+    std::vector<double> t;          // their absolute times: [2][recs.size()] (hi, lo)
+    std::vector<std::uint32_t> go;  // local lanes whose terminal-event callback continues
+    dev_ptr<unsigned char> d_buf;   // staging of records, times and lanes
+    std::size_t buf_bytes = 0;
+
+    unsigned char *buf(std::size_t bytes)
+    {
+        if (bytes > buf_bytes) {
+            buf_bytes = std::max(bytes, 2u * buf_bytes);
+            d_buf = dev_alloc<unsigned char>(buf_bytes);
+        }
+        return d_buf.get();
+    }
+};
+
+struct ev_loop {
+    hy_batch *b;
+    hy_event_callback cb;
+    void *user;
+    std::vector<ev_shard> sh; // one per shard of b
+    std::vector<hy_event_rec> recs;
+    std::vector<double> t_hi, t_lo;
+    std::vector<unsigned char> cont;
+    std::uint64_t iter = 0; // iterations taken
+    bool started = false;   // some iteration's bookkeeping ran in this call
+    unsigned done = 0;      // lanes at their target in the last iteration
+    bool nf = false;        // a lane went non-finite in the last iteration
+    bool stop = false;      // a terminal event without a callback, or whose callback returned false, fired
+
+    ev_loop(hy_batch *b_, hy_event_callback cb_, void *user_) : b(b_), cb(cb_), user(user_), sh(b_->shards.size()) {}
+
+    // One iteration of every shard: event step, callbacks (if there are records), terminal-event decisions,
+    // bookkeeping, then after_book(shard, i) and the flags read back.
+    void iterate(const std::function<void(shard &, std::size_t)> &after_book)
+    {
+        for_each_shard(b, [&](shard &s, std::size_t i) {
+            ev_shard &e = sh[i];
+            e.recs = s.ev_step(e.ls->L.dt_limit, 0);
+            const auto k = static_cast<std::uint32_t>(e.recs.size());
+            e.t.resize(2u * std::size_t(k));
+            if (k != 0u) {
+                unsigned char *buf = e.buf(k * (sizeof(hy_event_rec) + 2u * sizeof(double)));
+                auto *d_recs = reinterpret_cast<hy_event_rec *>(buf);
+                auto *d_t = reinterpret_cast<double *>(buf + std::size_t(k) * sizeof(hy_event_rec));
+                HY_CUDA_CHECK(cudaMemcpyAsync(d_recs, e.recs.data(), sizeof(hy_event_rec) * k, cudaMemcpyHostToDevice,
+                                              s.stream));
+                dev::k_ev_times<<<(k + 127u) / 128u, 128, 0, s.stream>>>(s.view(), d_recs, k, d_t, d_t + k);
+                HY_CUDA_CHECK(cudaGetLastError());
+                ++s.n_launches;
+                HY_CUDA_CHECK(cudaMemcpyAsync(e.t.data(), d_t, sizeof(double) * 2u * k, cudaMemcpyDeviceToHost, s.stream));
+                HY_CUDA_CHECK(cudaStreamSynchronize(s.stream));
+            }
+        });
+        // The shards' records one after the other, with the lanes of the whole batch (as hy_batch_step() lists them).
+        recs.clear();
+        t_hi.clear();
+        t_lo.clear();
+        for (std::size_t i = 0; i < sh.size(); ++i) {
+            const std::size_t k = sh[i].recs.size();
+            for (std::size_t j = 0; j < k; ++j) {
+                hy_event_rec r = sh[i].recs[j];
+                r.lane += b->off[i];
+                recs.push_back(r);
+                t_hi.push_back(sh[i].t[j]);
+                t_lo.push_back(sh[i].t[k + j]);
+            }
+        }
+        if (!recs.empty()) {
+            cont.assign(recs.size(), 0u);
+            const int r = cb(user, recs.data(), t_hi.data(), t_lo.data(), static_cast<std::uint32_t>(recs.size()),
+                             cont.data());
+            std::size_t k = 0;
+            for (auto &e : sh) {
+                e.go.clear();
+                for (const auto &rec : e.recs) {
+                    if (rec.terminal != 0) {
+                        if (cont[k] != 0u) {
+                            e.go.push_back(rec.lane);
+                        } else {
+                            stop = true;
+                        }
+                    }
+                    ++k;
+                }
+            }
+            // The decisions are applied whatever the callback returned, like the front ends' loops do lane by lane.
+            for_each_shard(b, [&](shard &s, std::size_t i) {
+                ev_shard &e = sh[i];
+                const auto n_go = static_cast<std::uint32_t>(e.go.size());
+                if (n_go != 0u) {
+                    auto *d_lanes = reinterpret_cast<std::uint32_t *>(e.buf(sizeof(std::uint32_t) * n_go));
+                    HY_CUDA_CHECK(cudaMemcpyAsync(d_lanes, e.go.data(), sizeof(std::uint32_t) * n_go,
+                                                  cudaMemcpyHostToDevice, s.stream));
+                    dev::k_ev_continue<<<(n_go + 127u) / 128u, 128, 0, s.stream>>>(s.view(), d_lanes, n_go);
+                    HY_CUDA_CHECK(cudaGetLastError());
+                    ++s.n_launches;
+                }
+                if (r < 0 && !started) {
+                    // Aborted before any bookkeeping: the per-lane results read as before the first step.
+                    dev::k_fill_outcome<<<(s.n + 255u) / 256u, 256, 0, s.stream>>>(s.d_prop_outcome, s.n, 0);
+                    dev::k_fill_double<<<(s.n + 255u) / 256u, 256, 0, s.stream>>>(s.d_prop_min_h, s.n, 0.);
+                    HY_CUDA_CHECK(cudaGetLastError());
+                }
+                HY_CUDA_CHECK(cudaStreamSynchronize(s.stream));
+            });
+            if (r < 0) {
+                throw callback_abort{};
+            }
+        }
+        for_each_shard(b, [&](shard &s, std::size_t i) {
+            sh[i].ls->book();
+            after_book(s, i);
+            sh[i].ls->read();
+        });
+        started = true;
+        done = 0u;
+        nf = false;
+        for (const auto &e : sh) {
+            done += e.ls->flags[0];
+            nf = nf || e.ls->flags[1] != 0u;
+        }
+        ++iter;
+    }
+    void iterate()
+    {
+        iterate([](shard &, std::size_t) {});
+    }
+
+    // propagate_until() from the lock-step states already initialised: iterations up to the loop's exits, every
+    // iteration that ends with finite states recorded by rec (single shard, on the shard's device) if given.
+    void run_until(std::uint64_t max_steps, hy_cout_rec *rec)
+    {
+        shard &s0 = *b->shards[0];
+        while (true) {
+            iterate();
+            if (nf) {
+                return; // non-finite state: this iteration is not recorded (:1462-1467)
+            }
+            if (rec != nullptr) {
+                // (The recorder allocates its slabs and times on the shard's device.)
+                device_guard guard(s0.device);
+                HY_CUDA_CHECK(cudaMemcpyAsync(rec->slot(), s0.d_tc, sizeof(double) * rec->tc_doubles,
+                                              cudaMemcpyDeviceToDevice, s0.stream));
+                rec->commit(s0);
+            }
+            if (stop || done == b->n) {
+                return;
+            }
+            if (iter == max_steps) {
+                for_each_shard(b, [&](shard &s, std::size_t) {
+                    dev::k_fill_outcome<<<(s.n + 255u) / 256u, 256, 0, s.stream>>>(s.d_prop_outcome, s.n,
+                                                                                    HY_OUTCOME_STEP_LIMIT);
+                    HY_CUDA_CHECK(cudaGetLastError());
+                    HY_CUDA_CHECK(cudaStreamSynchronize(s.stream));
+                });
+                return;
+            }
+        }
+    }
+};
+
+// The checks every event propagation makes on its batch and callback.
+void check_ev_batch(const hy_batch *b, hy_event_callback cb, const char *fn)
+{
+    if (b == nullptr || cb == nullptr) {
+        throw std::invalid_argument(std::string("Null pointer passed to ") + fn);
+    }
+    if (b->n_ev == 0u) {
+        throw std::invalid_argument(std::string(fn) + " needs a batch with event equations");
+    }
+    if (!b->ev_set) {
+        throw std::invalid_argument("hy_batch_set_events() must be called before stepping a batch with event equations");
+    }
+    for (const auto &s : b->shards) {
+        if (s->angles_on) {
+            throw hy::detail::not_implemented_error("The angle reducer does not run inside the propagation of a batch "
+                                                    "with event equations");
+        }
+    }
+}
+
+} // namespace
+
+int hy_batch_propagate_until_ev(hy_batch *b, const double *t_final_hi, const double *t_final_lo,
+                                const double *max_delta_t, uint64_t max_steps, hy_event_callback cb, void *user,
+                                hy_cout **c_out)
+{
+    try {
+        check_ev_batch(b, cb, "hy_batch_propagate_until_ev()");
+        if (t_final_hi == nullptr) {
+            throw std::invalid_argument("Null final times passed to hy_batch_propagate_until_ev()");
+        }
+        if (c_out != nullptr) {
+            *c_out = nullptr;
+            if (b->multi) {
+                throw hy::detail::not_implemented_error("Continuous output is not available on a multi-device batch");
+            }
+        }
+        check_prop_args(b->n, t_final_hi, t_final_lo, max_delta_t);
+        check_prop_times(b, t_final_hi, t_final_lo);
+        ev_loop L(b, cb, user);
+        for_each_shard(b, [&](shard &s, std::size_t i) {
+            const std::size_t off = b->off[i];
+            ev_shard &e = L.sh[i];
+            e.d_tf = dev_alloc<double>(2u * std::size_t(s.n));
+            HY_CUDA_CHECK(cudaMemcpyAsync(e.d_tf.get(), t_final_hi + off, sizeof(double) * s.n, cudaMemcpyHostToDevice,
+                                          s.stream));
+            if (t_final_lo != nullptr) {
+                HY_CUDA_CHECK(cudaMemcpyAsync(e.d_tf.get() + s.n, t_final_lo + off, sizeof(double) * s.n,
+                                              cudaMemcpyHostToDevice, s.stream));
+            }
+            e.ls = std::make_unique<lockstep>(s, e.d_tf.get(), t_final_lo != nullptr ? e.d_tf.get() + s.n : nullptr,
+                                              max_delta_t != nullptr ? max_delta_t + off : nullptr);
+            e.ls->init();
+            e.ls->read();
+        });
+        for (const auto &e : L.sh) {
+            if (e.ls->flags[2] != 0u) {
+                throw std::invalid_argument("The final time passed to the propagate_until() function of an adaptive "
+                                            "Taylor integrator in batch mode results in an overflow condition");
+            }
+        }
+        shard &s0 = *b->shards[0];
+        std::unique_ptr<hy_cout_rec> rec;
+        if (c_out != nullptr) {
+            device_guard guard(s0.device);
+            rec = std::make_unique<hy_cout_rec>(s0);
+        }
+        L.run_until(max_steps, rec.get());
+        if (rec != nullptr) {
+            device_guard guard(s0.device);
+            std::vector<unsigned char> forward(s0.n);
+            HY_CUDA_CHECK(cudaMemcpyAsync(forward.data(), L.sh[0].ls->L.t_dir, s0.n, cudaMemcpyDeviceToHost, s0.stream));
+            HY_CUDA_CHECK(cudaStreamSynchronize(s0.stream));
+            *c_out = rec->finish(s0, forward.data());
+            HY_CUDA_CHECK(cudaStreamSynchronize(s0.stream));
+        }
+        return HY_OK;
+    } catch (const callback_abort &) {
+        hy::detail::set_last_error("A host callback aborted the propagation");
+        return HY_ERR_CALLBACK;
+    } catch (...) {
+        return translate_exception();
+    }
+}
+
+int hy_batch_propagate_grid_ev(hy_batch *b, const double *grid, uint64_t n_pts, const double *max_delta_t,
+                               uint64_t max_steps, hy_event_callback cb, void *user, double *out)
+{
+    try {
+        check_ev_batch(b, cb, "hy_batch_propagate_grid_ev()");
+        if (grid == nullptr || out == nullptr) {
+            throw std::invalid_argument("Null pointer passed to hy_batch_propagate_grid_ev()");
+        }
+        if (b->multi) {
+            throw hy::detail::not_implemented_error("propagate_grid() is not available on a multi-device batch");
+        }
+        check_grid(b, grid, n_pts, max_delta_t);
+        shard &sh = *b->shards[0];
+        device_guard guard(sh.device);
+        const std::uint32_t n = sh.n;
+        const std::size_t n_out = static_cast<std::size_t>(n_pts) * sh.n_eq * n, state_doubles = std::size_t(sh.n_eq) * n;
+        const auto d_grid = dev_alloc<double>(n_pts * n), d_out = dev_alloc<double>(n_out);
+        const auto d_idx = dev_alloc<std::uint32_t>(n);
+        HY_CUDA_CHECK(cudaMemcpyAsync(d_grid.get(), grid, sizeof(double) * n_pts * n, cudaMemcpyHostToDevice, sh.stream));
+        dev::k_fill_double<<<static_cast<unsigned>((n_out + 255u) / 256u), 256, 0, sh.stream>>>(
+            d_out.get(), n_out, std::numeric_limits<double>::quiet_NaN());
+        HY_CUDA_CHECK(cudaGetLastError());
+        const unsigned gb = (n + 127u) / 128u;
+        const auto finish = [&]() {
+            HY_CUDA_CHECK(cudaMemcpyAsync(out, d_out.get(), sizeof(double) * n_out, cudaMemcpyDeviceToHost, sh.stream));
+            HY_CUDA_CHECK(cudaStreamSynchronize(sh.stream));
+            return HY_OK;
+        };
+
+        // Up to the first grid point, with the events and their callbacks (:1697-1706: propagate_until()).
+        ev_loop L(b, cb, user);
+        L.sh[0].ls = std::make_unique<lockstep>(sh, d_grid.get(), nullptr, max_delta_t);
+        L.sh[0].ls->init();
+        L.run_until(max_steps, nullptr);
+        {
+            std::vector<long long> oc(n);
+            HY_CUDA_CHECK(cudaMemcpyAsync(oc.data(), sh.d_prop_outcome, sizeof(long long) * n, cudaMemcpyDeviceToHost,
+                                          sh.stream));
+            HY_CUDA_CHECK(cudaStreamSynchronize(sh.stream));
+            if (std::any_of(oc.begin(), oc.end(), [](long long v) { return v != HY_OUTCOME_TIME_LIMIT; })) {
+                // Outcomes kept, counters reset (:1709-1722).
+                dev::k_fill_double<<<gb, 128, 0, sh.stream>>>(sh.d_prop_min_h, n, std::numeric_limits<double>::infinity());
+                dev::k_fill_double<<<gb, 128, 0, sh.stream>>>(sh.d_prop_max_h, n, 0.);
+                HY_CUDA_CHECK(cudaMemsetAsync(sh.d_prop_n_steps, 0, sizeof(unsigned long long) * n, sh.stream));
+                return finish();
+            }
+        }
+        HY_CUDA_CHECK(cudaMemcpyAsync(d_out.get(), sh.d_state, sizeof(double) * state_doubles, cudaMemcpyDeviceToDevice,
+                                      sh.stream));
+        // Grid point 0 is the state just copied: every cursor starts at 1.
+        const std::vector<std::uint32_t> first(n, 1u);
+        HY_CUDA_CHECK(cudaMemcpyAsync(d_idx.get(), first.data(), sizeof(std::uint32_t) * n, cudaMemcpyHostToDevice,
+                                      sh.stream));
+
+        // Then the lock-step loop towards the last grid point, sampling after every iteration.
+        L.sh[0].ls = std::make_unique<lockstep>(sh, d_grid.get() + (n_pts - 1u) * n, nullptr, max_delta_t);
+        lockstep &ls = *L.sh[0].ls;
+        const dev::grid_state G{d_grid.get(), static_cast<std::uint32_t>(n_pts), d_out.get(), d_idx.get(),
+                                ls.d_flags.get() + 3};
+        const auto sample = [&](shard &s, std::size_t) {
+            dev::k_grid_sample<<<dim3(gb, s.n_eq), 128, 0, s.stream>>>(s.prog, s.view(), G, ls.L);
+            dev::k_grid_advance<<<gb, 128, 0, s.stream>>>(s.view(), G, ls.L);
+            HY_CUDA_CHECK(cudaGetLastError());
+        };
+        ls.init();
+        sample(sh, 0);
+        ls.read();
+        if (ls.flags[2] != 0u) {
+            throw std::invalid_argument("The final time passed to the propagate_grid() function of an adaptive Taylor "
+                                        "integrator in batch mode results in an overflow condition");
+        }
+        L.iter = 0;
+        L.stop = false;
+        bool interrupted = false;
+        while (ls.flags[3] != 0u && !interrupted) {
+            L.iterate(sample);
+            if (L.nf) {
+                break; // non-finite state: nothing further is written (:1973-1978)
+            }
+            // A stopping terminal event ends the loop once the grid points of this step are written.
+            interrupted = L.stop;
+            if (L.iter == max_steps) {
+                dev::k_fill_outcome<<<(n + 255u) / 256u, 256, 0, sh.stream>>>(sh.d_prop_outcome, n,
+                                                                              HY_OUTCOME_STEP_LIMIT);
+                interrupted = true;
+            }
+        }
+        return finish();
+    } catch (const callback_abort &) {
+        hy::detail::set_last_error("A host callback aborted the propagation");
+        return HY_ERR_CALLBACK;
     } catch (...) {
         return translate_exception();
     }

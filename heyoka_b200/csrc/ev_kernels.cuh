@@ -675,6 +675,31 @@ __global__ void k_ev_filter(batch D, ev_args E)
     E.rec[i].live = live ? 1u : 0u;
 }
 
+// The absolute times of the records a device propagation calls back for (hy_batch_propagate_until_ev()): new time -
+// last_h + t in double-length arithmetic, as the front ends compute the time of a non-terminal event
+// (src/taylor_adaptive_batch.cpp:889). recs: the shard's live records, lanes local to the shard.
+__global__ void k_ev_times(batch D, const hy_event_rec *recs, std::uint32_t n_rec, double *t_hi, double *t_lo)
+{
+    const unsigned i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n_rec) {
+        return;
+    }
+    const hy_event_rec r = recs[i];
+    dfl t = dfl_add(dfl{D.t_hi[r.lane], D.t_lo[r.lane]}, dfl{-D.last_h[r.lane], 0.});
+    t = dfl_add(t, dfl{r.t, 0.});
+    t_hi[i] = t.hi;
+    t_lo[i] = t.lo;
+}
+
+// The lanes whose terminal-event callback asks to continue: outcome -idx - 1 -> idx (:958-969).
+__global__ void k_ev_continue(batch D, const std::uint32_t *lanes, std::uint32_t n)
+{
+    const unsigned i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < n) {
+        D.step_outcome[lanes[i]] = -D.step_outcome[lanes[i]] - 1;
+    }
+}
+
 // reset_cooldowns() for one lane or all of them (src/taylor_adaptive_batch.cpp:2300-2330).
 __global__ void k_ev_reset_cd(ev_args E, std::uint32_t n, std::uint32_t lane_or_all)
 {

@@ -150,6 +150,9 @@ struct taylor_adaptive_batch<double>::impl {
     // asks for them.
     bool lazy = false;
     bool host_new_state = true, host_new_pars = true, host_new_time = true;
+    // While the callbacks of a device event propagation run: the terminal-event decisions taken so far in the iteration
+    // (lane, outcome), which a step_res fetched from the device does not hold yet.
+    std::vector<std::pair<std::uint32_t, std::int64_t>> ev_decisions;
     bool dev_new_state = false, dev_new_time = false, dev_new_tc = false, dev_new_step = false, dev_new_prop = false;
     // The storage of the mirrors is page-locked in place (hy_host_pin()).
     std::vector<void *> pinned;
@@ -282,6 +285,9 @@ struct taylor_adaptive_batch<double>::impl {
             check(hy_batch_download_step_res(batch, oc.data(), tmp_a.data()));
             for (std::uint32_t i = 0; i < batch_size; ++i) {
                 step_res[i] = std::tuple{static_cast<taylor_outcome>(oc[i]), tmp_a[i]};
+            }
+            for (const auto &[lane, outcome] : ev_decisions) {
+                std::get<0>(step_res[lane]) = taylor_outcome{outcome};
             }
             dev_new_step = false;
         }
@@ -966,22 +972,49 @@ void taylor_adaptive_batch<double>::run_event_callbacks()
     std::vector<hy_event_rec> evs(n_ev);
     check(hy_batch_get_events(m.batch, evs.data(), n_ev));
     const auto t_hi = m.time_hi, t_lo = m.time_lo;
+    call_event_callbacks(
+        evs.data(), evs.size(),
+        [&](std::size_t k) {
+            // new_time - last_h + t in double-length arithmetic (:889).
+            const auto lane = evs[k].lane;
+            return dfl_add(dfl_sub(dfl{t_hi[lane], t_lo[lane]}, dfl{m.last_h[lane], 0.}), dfl{evs[k].t, 0.}).hi;
+        },
+        [&](std::size_t k, bool ret) {
+            const auto ev_idx = static_cast<std::int64_t>(evs[k].idx);
+            m.step_res[evs[k].lane] = std::tuple{taylor_outcome{ret ? ev_idx : (-ev_idx - 1)}, m.last_h[evs[k].lane]};
+        });
+    const auto same = [](double a, double b) { return a == b || (std::isnan(a) && std::isnan(b)); };
+    for (std::uint32_t i = 0; i < m.batch_size; ++i) {
+        if (!same(m.time_hi[i], t_hi[i]) || !same(m.time_lo[i], t_lo[i])) {
+            throw std::runtime_error("The invocation of one or more event callbacks resulted in the alteration of the "
+                                     "time coordinate of the integrator at the batch index "
+                                     + std::to_string(i) + " - this is not supported");
+        }
+    }
+}
+
+// The callbacks of one step's events, evs as hy_batch_get_events() lists them: per lane the non-terminal events, then
+// the terminal one. nt_time(k): the absolute time of record k; decide(k, ret): the decision of the terminal event k
+// whose callback returned (ret: continue). A lane stops at its first exception, the other lanes go on; the exceptions
+// are rethrown at the end as the reference does.
+void taylor_adaptive_batch<double>::call_event_callbacks(const hy_event_rec *evs, std::size_t n,
+                                                         const std::function<double(std::size_t)> &nt_time,
+                                                         const std::function<void(std::size_t, bool)> &decide)
+{
+    auto &m = *m_impl;
     std::vector<std::pair<std::uint32_t, std::exception_ptr>> cb_eptrs;
-    for (std::size_t k = 0; k < evs.size();) {
+    for (std::size_t k = 0; k < n;) {
         const auto lane = evs[k].lane;
         std::size_t end = k;
-        while (end < evs.size() && evs[end].lane == lane) {
+        while (end < n && evs[end].lane == lane) {
             ++end;
         }
-        const double h = m.last_h[lane];
         bool nt_cb_exception = false;
         std::size_t j = k;
         for (; j < end && evs[j].terminal == 0; ++j) {
             auto &cb = m.ntes[evs[j].idx].get_callback();
-            // new_time - last_h + t in double-length arithmetic (:889).
-            const auto tm = dfl_add(dfl_sub(dfl{t_hi[lane], t_lo[lane]}, dfl{h, 0.}), dfl{evs[j].t, 0.}).hi;
             try {
-                cb(*this, tm, evs[j].d_sgn, lane);
+                cb(*this, nt_time(j), evs[j].d_sgn, lane);
             } catch (...) {
                 cb_eptrs.emplace_back(lane, std::current_exception());
                 nt_cb_exception = true;
@@ -1003,8 +1036,7 @@ void taylor_adaptive_batch<double>::run_event_callbacks()
                         }
                     }
                     if (!thrown) {
-                        const auto ev_idx = static_cast<std::int64_t>(evs[j].idx);
-                        m.step_res[lane] = std::tuple{taylor_outcome{te_cb_ret ? ev_idx : (-ev_idx - 1)}, h};
+                        decide(j, te_cb_ret);
                     }
                     break;
                 }
@@ -1032,13 +1064,93 @@ void taylor_adaptive_batch<double>::run_event_callbacks()
         }
         throw std::runtime_error(exc_msg);
     }
-    const auto same = [](double a, double b) { return a == b || (std::isnan(a) && std::isnan(b)); };
-    for (std::uint32_t i = 0; i < m.batch_size; ++i) {
-        if (!same(m.time_hi[i], t_hi[i]) || !same(m.time_lo[i], t_lo[i])) {
-            throw std::runtime_error("The invocation of one or more event callbacks resulted in the alteration of the "
-                                     "time coordinate of the integrator at the batch index "
-                                     + std::to_string(i) + " - this is not supported");
+}
+
+namespace
+{
+struct device_ev_hook {
+    taylor_adaptive_batch<double> *self;
+    bool was_lazy;
+    std::exception_ptr err;
+};
+} // namespace
+
+// The callbacks of one iteration of hy_batch_propagate_until_ev() / hy_batch_propagate_grid_ev(). The host_sync::lazy
+// machinery applies to the callback scope: every mirror is marked stale and the first access fetches it; afterwards
+// the state and parameters a callback could have written go back to the device, as the host loop's next push() would
+// send them. The time must not change: if a callback read or set it, it is compared with the device's.
+int taylor_adaptive_batch<double>::device_event_callbacks(void *user, const hy_event_rec *recs, const double *t_hi,
+                                                          const double *, std::uint32_t n_rec, unsigned char *cont)
+{
+    auto &h = *static_cast<device_ev_hook *>(user);
+    auto &m = *h.self->m_impl;
+    m.lazy = true;
+    m.dev_new_state = m.dev_new_time = m.dev_new_tc = m.dev_new_step = m.dev_new_prop = true;
+    m.tc_valid = true;
+    m.host_new_state = m.host_new_pars = m.host_new_time = false;
+    m.ev_decisions.clear();
+    try {
+        try {
+            h.self->call_event_callbacks(
+                recs, n_rec, [t_hi](std::size_t k) { return t_hi[k]; },
+                [&](std::size_t k, bool ret) {
+                    const auto ev_idx = static_cast<std::int64_t>(recs[k].idx);
+                    const auto outcome = ret ? ev_idx : (-ev_idx - 1);
+                    cont[k] = ret ? 1u : 0u;
+                    m.ev_decisions.emplace_back(recs[k].lane, outcome);
+                    if (!m.dev_new_step) {
+                        std::get<0>(m.step_res[recs[k].lane]) = taylor_outcome{outcome};
+                    }
+                });
+        } catch (...) {
+            if (m.host_new_state || m.host_new_pars) {
+                check(hy_batch_upload(m.batch, m.host_new_state ? m.state.data() : nullptr,
+                                      m.host_new_pars && m.n_pars != 0u ? m.pars.data() : nullptr, nullptr, nullptr));
+            }
+            throw;
         }
+        if (m.host_new_state || m.host_new_pars) {
+            check(hy_batch_upload(m.batch, m.host_new_state ? m.state.data() : nullptr,
+                                  m.host_new_pars && m.n_pars != 0u ? m.pars.data() : nullptr, nullptr, nullptr));
+            m.host_new_state = m.host_new_pars = false;
+        }
+        if (m.host_new_time || !m.dev_new_time) {
+            std::vector<double> dh(m.batch_size), dl(m.batch_size);
+            check(hy_batch_download(m.batch, nullptr, dh.data(), dl.data(), nullptr));
+            const auto same = [](double a, double b) { return a == b || (std::isnan(a) && std::isnan(b)); };
+            for (std::uint32_t i = 0; i < m.batch_size; ++i) {
+                if (!same(m.time_hi[i], dh[i]) || !same(m.time_lo[i], dl[i])) {
+                    throw std::runtime_error("The invocation of one or more event callbacks resulted in the alteration "
+                                             "of the time coordinate of the integrator at the batch index "
+                                             + std::to_string(i) + " - this is not supported");
+                }
+            }
+        }
+        m.ev_decisions.clear();
+        return 1;
+    } catch (...) {
+        m.ev_decisions.clear();
+        h.err = std::current_exception();
+        return -1;
+    }
+}
+
+// After a device event propagation: the synchronisation mode of the integrator again, and the mirrors marked as held by
+// the device. ok = false (a callback raised): the mirrors the last callbacks fetched keep what the callbacks left in
+// them, as after the host loop.
+void taylor_adaptive_batch<double>::end_device_event_call(bool ok)
+{
+    auto &m = *m_impl;
+    const bool keep_state = !ok && !m.dev_new_state, keep_time = !ok && !m.dev_new_time, keep_tc = !ok && !m.dev_new_tc,
+               keep_step = !ok && !m.dev_new_step, keep_prop = !ok && !m.dev_new_prop;
+    m.dev_new_state = !keep_state;
+    m.dev_new_time = !keep_time;
+    m.dev_new_tc = !keep_tc;
+    m.dev_new_step = !keep_step;
+    m.dev_new_prop = !keep_prop;
+    m.tc_valid = true;
+    if (!m.lazy) {
+        m.refresh_all();
     }
 }
 
@@ -1310,6 +1422,22 @@ taylor_adaptive_batch<double>::propagate_grid_impl(const std::vector<double> &gr
             return res;
         }
     }
+    if (!o.cb && with_events() && m.devices.empty()) {
+        // Events without a step callback: the lock-step loop on the device (hy_batch_propagate_grid_ev()).
+        std::vector<double> retval(grid.size() * m.dim);
+        m.push();
+        device_ev_hook hook{this, m.lazy, nullptr};
+        const int st = hy_batch_propagate_grid_ev(m.batch, grid.data(), grid.size() / n,
+                                                  o.max_delta_t.empty() ? nullptr : o.max_delta_t.data(), o.max_steps,
+                                                  &taylor_adaptive_batch::device_event_callbacks, &hook, retval.data());
+        m.lazy = hook.was_lazy;
+        end_device_event_call(!hook.err);
+        if (hook.err) {
+            std::rethrow_exception(hook.err);
+        }
+        check(st);
+        return {std::move(o.cb), std::move(retval)};
+    }
     if (o.cb || with_events() || !m.devices.empty()) {
         // A step callback (or events, whose callbacks also run on the host) after every step: the reference's loop on the
         // host, one device step per iteration. A batch sharded over several devices takes it too (the grid is sampled
@@ -1534,6 +1662,28 @@ taylor_adaptive_batch<double>::propagate_until_impl(const std::vector<double> &h
             std::get<1>(res) = std::move(cb);
             return res;
         }
+    }
+
+    if (!o.cb && with_events()) {
+        // Events without a step callback: the lock-step loop on the device (hy_batch_propagate_until_ev()); the event
+        // callbacks run on the host in the iterations that have events.
+        m.push();
+        device_ev_hook hook{this, m.lazy, nullptr};
+        hy_cout *co = nullptr;
+        const int st = hy_batch_propagate_until_ev(m.batch, hi.data(), lo.data(), mdt, o.max_steps,
+                                                   &taylor_adaptive_batch::device_event_callbacks, &hook,
+                                                   o.c_output ? &co : nullptr);
+        m.lazy = hook.was_lazy;
+        end_device_event_call(!hook.err);
+        if (hook.err) {
+            std::rethrow_exception(hook.err);
+        }
+        check(st);
+        std::optional<continuous_output_batch<double>> ret;
+        if (co != nullptr) {
+            ret.emplace(co, n, m.dim, m.order);
+        }
+        return {std::move(ret), std::move(o.cb)};
     }
 
     if (o.c_output && !with_events()) {

@@ -366,8 +366,9 @@ int hy_batch_eval_taylor_map(hy_batch *, uint32_t n_orig_sv, uint32_t n_args, co
  *    hy_batch_step() is an event step: jet (Taylor coefficients always written; rows n_eq.. of the device tc array hold
  *    the event equations), detection, propagation cut at the first terminal event of each lane, cooldowns. Callbacks are
  *    the caller's: it reads the detected events back and patches the outcome of a terminal event whose callback asks to
- *    continue (-idx - 1 -> idx). hy_batch_propagate_*() refuse such a batch: the front ends run the reference's
- *    lock-step loop over hy_batch_step() (a callback per step forces a synchronisation anyway).
+ *    continue (-idx - 1 -> idx). hy_batch_propagate_until{,_host,_dev,_cout,_cout_cb}() and hy_batch_propagate_grid()
+ *    refuse such a batch: it is propagated by hy_batch_propagate_until_ev() / hy_batch_propagate_grid_ev() below, or by
+ *    a caller's own lock-step loop over hy_batch_step() (the front ends' loop for a step callback together with events).
  * ---------------------------------------------------------------------------------------------- */
 typedef struct hy_event_rec {
     uint32_t lane;    /* batch index                                                         */
@@ -393,6 +394,31 @@ int hy_batch_get_cooldowns(hy_batch *, uint8_t *active, double *spent, double *c
 /* Restores a cooldown state (copies of an integrator carry the cooldowns of the original: the reference copies
  * m_te_cooldowns, src/detail/event_detection.cpp:1622-1645). */
 int hy_batch_set_cooldowns(hy_batch *, const uint8_t *active, const double *spent, const double *cooldown);
+
+/* Propagation of a batch with event equations on the device: the reference's lock-step loop of propagate_until() /
+ * propagate_grid() (src/taylor_adaptive_batch.cpp:1372-1527, :1696-2053) over event steps, with the step limits and
+ * the bookkeeping kept on the device. The callback runs on the host once per iteration in which some lane has event
+ * records, never otherwise. It receives the n_rec records of the whole batch in the order of hy_batch_get_events()
+ * (lanes ascending; per lane the non-terminal events by |t|, then the terminal one), with t_hi / t_lo[k] the absolute
+ * time of record k (time after the step - last_h + t, in double-length arithmetic). For every terminal record k it sets
+ * cont[k] != 0 to continue (outcome -idx - 1 -> idx) or leaves 0 to stop; the other bytes are ignored. Return value:
+ * > 0 go on, < 0 abort with HY_ERR_CALLBACK (the decisions written so far are applied; the iteration's bookkeeping is
+ * not done, and an abort in the first iteration leaves the per-lane results at outcome 0, min_h = max_h = 0, 0 steps).
+ * The batch is synchronised while the callback runs: it may download / upload state and parameters (not the time).
+ * Exits as in the reference: a non-finite state in any lane (after that iteration's bookkeeping), a stopping terminal
+ * event in any lane (a terminal record left at 0), max_steps iterations (every outcome becomes step_limit), every lane
+ * at its target. The Taylor coefficients are always written. The angle reducer (hy_batch_set_angles()) is refused.
+ * hy_batch_propagate_until_ev(): any number of shards; c_out (may be NULL) receives the continuous output of the call
+ * (single device only), *c_out = NULL if no iteration completed. Results via hy_batch_download_prop_res().
+ * hy_batch_propagate_grid_ev(): single device; the initial propagation to grid[0] runs the same loop with the same
+ * callback; out[n_pts * n_eq * batch] as hy_batch_propagate_grid(). */
+typedef int (*hy_event_callback)(void *user, const hy_event_rec *recs, const double *t_hi, const double *t_lo,
+                                 uint32_t n_rec, unsigned char *cont);
+int hy_batch_propagate_until_ev(hy_batch *, const double *t_final_hi, const double *t_final_lo,
+                                const double *max_delta_t, uint64_t max_steps, hy_event_callback cb, void *user,
+                                hy_cout **c_out);
+int hy_batch_propagate_grid_ev(hy_batch *, const double *grid, uint64_t n_pts, const double *max_delta_t,
+                               uint64_t max_steps, hy_event_callback cb, void *user, double *out);
 
 /* The angle reducer (callback::angle_reducer, include/heyoka_b200/callback.hpp). hy_batch_set_angles() sets the state
  * variables (indices into the state rows) that the propagate entry points reduce into [0, 2pi) after every step, on

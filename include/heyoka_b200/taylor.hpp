@@ -256,6 +256,12 @@ private:
     void finalise_ctor(const var_ode_sys &, std::vector<double>, std::uint32_t, ctor_opts);
     void step_impl(const std::vector<double> *, bool backward, bool wtc);
     void run_event_callbacks();
+    void call_event_callbacks(const hy_event_rec *, std::size_t, const std::function<double(std::size_t)> &,
+                              const std::function<void(std::size_t, bool)> &);
+    // The hy_event_callback of the device event propagations; user: a device_ev_hook (taylor_adaptive_batch.cpp).
+    static int device_event_callbacks(void *user, const hy_event_rec *, const double *t_hi, const double *t_lo,
+                                      std::uint32_t n_rec, unsigned char *cont);
+    void end_device_event_call(bool ok);
     std::tuple<std::optional<continuous_output_batch<double>>, step_callback_batch<double>>
     propagate_until_impl(const std::vector<double> &hi, const std::vector<double> &lo, prop_opts);
     std::tuple<step_callback_batch<double>, std::vector<double>> propagate_grid_impl(const std::vector<double> &,
