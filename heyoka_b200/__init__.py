@@ -1259,13 +1259,13 @@ class taylor_adaptive_batch:
                 self._prop_res = [(STEP_LIMIT,) + r[1:] for r in self._prop_res]
                 return finish()
 
-    def _device_angles(self, callback, grid=False):
+    def _device_angles(self, callback):
         """The state-row indices of an angle reducer passed as callback (checked before any step, like the reference's
         pre_hook()) when the reduction can run on the device, else None. A wrapped reducer is an ordinary callback."""
         if not isinstance(callback, _callback.angle_reducer):
             return None
         idx = callback.sv_indices(self)
-        if self._with_events or (grid and self._b.n_shards != 0):
+        if self._with_events:
             return None
         return idx if self._b.kernel_info()["tape"] in ("hbm", "smem", "global", "global-cta") else None
 
@@ -1356,7 +1356,7 @@ class taylor_adaptive_batch:
                 raise ValueError("Invalid number of max timesteps specified in a Taylor integrator in batch mode: the "
                                  "batch size is %d, but the number of specified timesteps is %d" % (n, md.size))
             max_delta_t = np.ascontiguousarray(md)
-        angles = self._device_angles(callback, grid=True)
+        angles = self._device_angles(callback)
         if angles is not None:
             # The angle reducer on the device, inside the grid loop.
             self._b.set_angles(angles)
@@ -1364,11 +1364,11 @@ class taylor_adaptive_batch:
                 return self.propagate_grid(g.reshape(-1, n), max_steps=max_steps, max_delta_t=max_delta_t)
             finally:
                 self._b.set_angles([])
-        if self._device_events(callback) and self._b.n_shards == 0:
+        if self._device_events(callback):
             return self._propagate_grid_events(g.reshape(-1, n), max_delta_t, max_steps)
-        if self._with_events or callback is not None or self._b.n_shards != 0:
-            # (Host loop: events and step callbacks are host code; a batch sharded over several devices samples its grid
-            # through the dense output of its shards.)
+        if self._with_events or callback is not None:
+            # (Host loop: a step callback other than the angle reducer is host code, and so are the event callbacks
+            # that run beside it.)
             return self._propagate_grid_host(g.reshape(-1, n), max_delta_t, max_steps, callback)
         self._push()
         out = self._b.propagate_grid(g.reshape(-1, n), max_delta_t, max_steps)

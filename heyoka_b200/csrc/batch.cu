@@ -2215,7 +2215,8 @@ int hy_batch_propagate_until_dev(hy_batch *b, const double *d_t_final_hi, const 
 // propagate_grid() (src/taylor_adaptive_batch.cpp:1545-2055). The reference's algorithm is kept as it is: an
 // initial propagate_until(grid[0]) with write_tc, then lock-step iterations of {dense output at every grid point
 // covered by the last step; one step clamped to the last grid point}. The per-lane work runs on the device (one
-// step launch + three small kernels per iteration); the host only reads the loop flags.
+// step launch + three small kernels per iteration); the host only reads the loop flags, and combines those of the
+// shards of a sharded batch.
 namespace
 {
 
@@ -2387,6 +2388,157 @@ struct lockstep {
     }
 };
 
+// propagate_grid() on every shard of a batch: per shard its columns of the grid, its block of the output, its cursors
+// and the lock-step state of the loop towards the last grid point. The reference's loop runs over the whole batch, so
+// the shards run in lock-step: every shard takes every iteration while some lane of some shard has grid points left (a
+// shard whose lanes are all at their target takes zero-length steps, as those lanes do inside one device), and an
+// iteration in which a lane of any shard goes non-finite is sampled by no shard.
+struct grid_run {
+    struct part {
+        dev_ptr<double> d_grid, d_out; // [n_pts][n], [n_pts][n_eq][n]
+        dev_ptr<std::uint32_t> d_idx;
+        std::shared_ptr<lockstep> ls; // (shared with the event loop's shard state)
+    };
+    hy_batch *b;
+    std::uint64_t n_pts;
+    const double *max_delta_t;
+    std::vector<part> p; // one per shard of b
+
+    // Stages the grid by column and fills every shard's output with NaN.
+    grid_run(hy_batch *b_, const double *grid, std::uint64_t n_pts_, const double *max_delta_t_)
+        : b(b_), n_pts(n_pts_), max_delta_t(max_delta_t_), p(b_->shards.size())
+    {
+        for_each_shard(b, [&](shard &s, std::size_t i) {
+            const std::size_t n_out = static_cast<std::size_t>(n_pts) * s.n_eq * s.n;
+            p[i].d_grid = dev_alloc<double>(n_pts * s.n);
+            p[i].d_out = dev_alloc<double>(n_out);
+            p[i].d_idx = dev_alloc<std::uint32_t>(s.n);
+            rows_h2d(s, p[i].d_grid.get(), grid, n_pts, b->n, b->off[i]);
+            dev::k_fill_double<<<static_cast<unsigned>((n_out + 255u) / 256u), 256, 0, s.stream>>>(
+                p[i].d_out.get(), n_out, std::numeric_limits<double>::quiet_NaN());
+            HY_CUDA_CHECK(cudaGetLastError());
+            HY_CUDA_CHECK(cudaStreamSynchronize(s.stream));
+        });
+    }
+    const double *mdt(std::size_t i) const
+    {
+        return max_delta_t != nullptr ? max_delta_t + b->off[i] : nullptr;
+    }
+    // After the propagation to grid[0]: whether every lane of every shard reached it. If not, the counters are reset
+    // and the outcomes kept (:1709-1722).
+    bool first_leg_done()
+    {
+        std::vector<long long> oc(b->n);
+        for_each_shard(b, [&](shard &s, std::size_t i) {
+            rows_d2h(s, oc.data(), s.d_prop_outcome, 1u, b->n, b->off[i]);
+            HY_CUDA_CHECK(cudaStreamSynchronize(s.stream));
+        });
+        if (std::all_of(oc.begin(), oc.end(), [](long long v) { return v == HY_OUTCOME_TIME_LIMIT; })) {
+            return true;
+        }
+        for_each_shard(b, [&](shard &s, std::size_t) {
+            const unsigned gb = (s.n + 127u) / 128u;
+            dev::k_fill_double<<<gb, 128, 0, s.stream>>>(s.d_prop_min_h, s.n, std::numeric_limits<double>::infinity());
+            dev::k_fill_double<<<gb, 128, 0, s.stream>>>(s.d_prop_max_h, s.n, 0.);
+            HY_CUDA_CHECK(cudaGetLastError());
+            HY_CUDA_CHECK(cudaMemsetAsync(s.d_prop_n_steps, 0, sizeof(unsigned long long) * s.n, s.stream));
+            HY_CUDA_CHECK(cudaStreamSynchronize(s.stream));
+        });
+        return false;
+    }
+    // Grid point 0 is the current state, every cursor starts at 1; the lock-step states towards the last grid point
+    // (each shard's reduced rows: angles[i]), and the grid points the zero-length interval before the first step covers.
+    void start(const std::vector<const unsigned char *> &angles)
+    {
+        for_each_shard(b, [&](shard &s, std::size_t i) {
+            part &q = p[i];
+            HY_CUDA_CHECK(cudaMemcpyAsync(q.d_out.get(), s.d_state, sizeof(double) * s.n_eq * s.n,
+                                          cudaMemcpyDeviceToDevice, s.stream));
+            const std::vector<std::uint32_t> first(s.n, 1u);
+            HY_CUDA_CHECK(cudaMemcpyAsync(q.d_idx.get(), first.data(), sizeof(std::uint32_t) * s.n,
+                                          cudaMemcpyHostToDevice, s.stream));
+            q.ls = std::make_shared<lockstep>(s, q.d_grid.get() + (n_pts - 1u) * s.n, nullptr, mdt(i));
+            q.ls->angles = angles[i];
+            q.ls->init();
+            sample(s, i);
+            q.ls->read();
+        });
+        for (const auto &q : p) {
+            if (q.ls->flags[2] != 0u) {
+                throw std::invalid_argument("The final time passed to the propagate_grid() function of an adaptive "
+                                            "Taylor integrator in batch mode results in an overflow condition");
+            }
+        }
+    }
+    // Dense output at the grid points the shard's last step covered, and the cursors past them. The word the lock-step
+    // state leaves to its caller is set when some lane has grid points left.
+    void sample(shard &s, std::size_t i)
+    {
+        const part &q = p[i];
+        const dev::grid_state G{q.d_grid.get(), static_cast<std::uint32_t>(n_pts), q.d_out.get(), q.d_idx.get(),
+                                q.ls->d_flags.get() + 3};
+        const unsigned gb = q.ls->blocks();
+        dev::k_grid_sample<<<dim3(gb, s.n_eq), 128, 0, s.stream>>>(s.prog, s.view(), G, q.ls->L);
+        dev::k_grid_advance<<<gb, 128, 0, s.stream>>>(s.view(), G, q.ls->L);
+        HY_CUDA_CHECK(cudaGetLastError());
+    }
+    bool any_flag(unsigned w) const
+    {
+        return std::any_of(p.begin(), p.end(), [w](const part &q) { return q.ls->flags[w] != 0u; });
+    }
+    // The lock-step loop (:1770-2053). iterate(hook) takes one iteration on every shard - step, bookkeeping, then
+    // hook(shard, i), then the flags read back - and returns true when it must be the last one (a stopping terminal
+    // event). One shard samples inside the hook, where the kernels' own check of the non-finite flag is batch-wide: one
+    // read-back per iteration. More shards combine their non-finite flags on the host first, then sample and read the
+    // flags again.
+    using shard_fn = std::function<void(shard &, std::size_t)>;
+    void loop(std::uint64_t max_steps, const std::function<bool(const shard_fn &)> &iterate)
+    {
+        const bool one = p.size() == 1u;
+        const shard_fn hook = [&](shard &s, std::size_t i) {
+            if (one) {
+                sample(s, i);
+            }
+        };
+        std::uint64_t iter = 0;
+        while (any_flag(3)) {
+            const bool stop = iterate(hook);
+            if (any_flag(1)) {
+                // Non-finite state: nothing further is written, and the reduction of this step is undone (:1973-1978).
+                for_each_shard(b, [&](shard &, std::size_t i) { p[i].ls->undo_reduction(); });
+                return;
+            }
+            if (!one) {
+                for_each_shard(b, [&](shard &s, std::size_t i) {
+                    sample(s, i);
+                    p[i].ls->read();
+                });
+            }
+            if (++iter == max_steps) {
+                for_each_shard(b, [&](shard &s, std::size_t) {
+                    dev::k_fill_outcome<<<(s.n + 255u) / 256u, 256, 0, s.stream>>>(s.d_prop_outcome, s.n,
+                                                                                    HY_OUTCOME_STEP_LIMIT);
+                    HY_CUDA_CHECK(cudaGetLastError());
+                    HY_CUDA_CHECK(cudaStreamSynchronize(s.stream));
+                });
+                return;
+            }
+            if (stop) {
+                return; // once the grid points of this step are written
+            }
+        }
+    }
+    // Every shard's block of the output into the caller's [n_pts][n_eq][batch] array.
+    int finish(double *out)
+    {
+        for_each_shard(b, [&](shard &s, std::size_t i) {
+            rows_d2h(s, out, p[i].d_out.get(), static_cast<std::size_t>(n_pts) * s.n_eq, b->n, b->off[i]);
+            HY_CUDA_CHECK(cudaStreamSynchronize(s.stream));
+        });
+        return HY_OK;
+    }
+};
+
 } // namespace
 
 int hy_batch_check_grid(hy_batch *b, const double *grid, uint64_t n_pts, const double *max_delta_t)
@@ -2410,86 +2562,29 @@ int hy_batch_propagate_grid(hy_batch *b, const double *grid, uint64_t n_pts, con
         if (b == nullptr || grid == nullptr || out == nullptr) {
             throw std::invalid_argument("Null pointer passed to hy_batch_propagate_grid()");
         }
-        if (b->multi) {
-            throw hy::detail::not_implemented_error("propagate_grid() is not available on a multi-device batch");
-        }
         check_grid(b, grid, n_pts, max_delta_t);
-        shard &sh = *b->shards[0];
-        device_guard guard(sh.device);
-        const std::uint32_t n = sh.n;
-        const unsigned char *angles = sh.prop_angles();
-
-        const std::size_t n_out = static_cast<std::size_t>(n_pts) * sh.n_eq * n, state_doubles = std::size_t(sh.n_eq) * n;
-        const auto d_grid = dev_alloc<double>(n_pts * n), d_out = dev_alloc<double>(n_out);
-        const auto d_idx = dev_alloc<std::uint32_t>(n);
-        HY_CUDA_CHECK(cudaMemcpyAsync(d_grid.get(), grid, sizeof(double) * n_pts * n, cudaMemcpyHostToDevice, sh.stream));
-        // The target of every lane is its last grid point.
-        lockstep ls(sh, d_grid.get() + (n_pts - 1u) * n, nullptr, max_delta_t);
-        ls.angles = angles;
-        dev::k_fill_double<<<static_cast<unsigned>((n_out + 255u) / 256u), 256, 0, sh.stream>>>(
-            d_out.get(), n_out, std::numeric_limits<double>::quiet_NaN());
-        HY_CUDA_CHECK(cudaGetLastError());
-        const unsigned gb = ls.blocks();
-        const auto finish = [&]() {
-            HY_CUDA_CHECK(cudaMemcpyAsync(out, d_out.get(), sizeof(double) * n_out, cudaMemcpyDeviceToHost, sh.stream));
-            HY_CUDA_CHECK(cudaStreamSynchronize(sh.stream));
-            return HY_OK;
-        };
+        std::vector<const unsigned char *> angles(b->shards.size());
+        for (std::size_t i = 0; i < b->shards.size(); ++i) {
+            angles[i] = b->shards[i]->prop_angles();
+        }
+        grid_run G(b, grid, n_pts, max_delta_t);
 
         // Up to the first grid point (a zero-length step when the time is already there: it brings the Taylor
         // coefficients up to date), :1697-1706. The reference calls no step callback there: no reduction.
-        {
-            propagate(b, d_grid.get(), nullptr, ls.L.max_delta_t, 1, max_steps, 1, nullptr, false);
-            std::vector<long long> oc(n);
-            HY_CUDA_CHECK(cudaMemcpyAsync(oc.data(), sh.d_prop_outcome, sizeof(long long) * n, cudaMemcpyDeviceToHost,
-                                          sh.stream));
-            HY_CUDA_CHECK(cudaStreamSynchronize(sh.stream));
-            if (std::any_of(oc.begin(), oc.end(), [](long long v) { return v != HY_OUTCOME_TIME_LIMIT; })) {
-                // Outcomes kept, counters reset (:1709-1722).
-                dev::k_fill_double<<<gb, 128, 0, sh.stream>>>(sh.d_prop_min_h, n, std::numeric_limits<double>::infinity());
-                dev::k_fill_double<<<gb, 128, 0, sh.stream>>>(sh.d_prop_max_h, n, 0.);
-                HY_CUDA_CHECK(cudaMemsetAsync(sh.d_prop_n_steps, 0, sizeof(unsigned long long) * n, sh.stream));
-                return finish();
-            }
+        propagate(b, grid, nullptr, max_delta_t, 0, max_steps, 1, nullptr, false);
+        if (!G.first_leg_done()) {
+            return G.finish(out);
         }
-        HY_CUDA_CHECK(cudaMemcpyAsync(d_out.get(), sh.d_state, sizeof(double) * state_doubles, cudaMemcpyDeviceToDevice,
-                                      sh.stream));
-        // Grid point 0 is the state just copied: every cursor starts at 1.
-        const std::vector<std::uint32_t> first(n, 1u);
-        HY_CUDA_CHECK(cudaMemcpyAsync(d_idx.get(), first.data(), sizeof(std::uint32_t) * n, cudaMemcpyHostToDevice,
-                                      sh.stream));
-
-        // The word the lock-step state leaves to its caller says whether some lane has grid points left.
-        const dev::grid_state G{d_grid.get(), static_cast<std::uint32_t>(n_pts), d_out.get(), d_idx.get(),
-                                ls.d_flags.get() + 3};
-        ls.init();
-        dev::k_grid_sample<<<dim3(gb, sh.n_eq), 128, 0, sh.stream>>>(sh.prog, sh.view(), G, ls.L);
-        dev::k_grid_advance<<<gb, 128, 0, sh.stream>>>(sh.view(), G, ls.L);
-        HY_CUDA_CHECK(cudaGetLastError());
-        ls.read();
-        if (ls.flags[2] != 0u) {
-            throw std::invalid_argument("The final time passed to the propagate_grid() function of an adaptive Taylor "
-                                        "integrator in batch mode results in an overflow condition");
-        }
-        std::uint64_t iter = 0;
-        bool interrupted = false;
-        while (ls.flags[3] != 0u && !interrupted) {
-            ls.iterate();
-            dev::k_grid_sample<<<dim3(gb, sh.n_eq), 128, 0, sh.stream>>>(sh.prog, sh.view(), G, ls.L);
-            dev::k_grid_advance<<<gb, 128, 0, sh.stream>>>(sh.view(), G, ls.L);
-            HY_CUDA_CHECK(cudaGetLastError());
-            ls.read();
-            if (ls.flags[1] != 0u) {
-                ls.undo_reduction();
-                break; // non-finite state: nothing further is written (:1973-1978)
-            }
-            if (++iter == max_steps) {
-                dev::k_fill_outcome<<<(n + 255u) / 256u, 256, 0, sh.stream>>>(sh.d_prop_outcome, n,
-                                                                              HY_OUTCOME_STEP_LIMIT);
-                interrupted = true;
-            }
-        }
-        return finish();
+        G.start(angles);
+        G.loop(max_steps, [&](const grid_run::shard_fn &hook) {
+            for_each_shard(b, [&](shard &s, std::size_t i) {
+                G.p[i].ls->iterate();
+                hook(s, i);
+                G.p[i].ls->read();
+            });
+            return false;
+        });
+        return G.finish(out);
     } catch (...) {
         return translate_exception();
     }
@@ -2794,7 +2889,7 @@ namespace
 {
 
 struct ev_shard {
-    std::unique_ptr<lockstep> ls;
+    std::shared_ptr<lockstep> ls;
     dev_ptr<double> d_tf;          // target times of propagate_until() (hi, lo)
     std::vector<hy_event_rec> recs; // live records of the iteration, lanes local to the shard
     std::vector<double> t;          // their absolute times: [2][recs.size()] (hi, lo)
@@ -3008,7 +3103,7 @@ int hy_batch_propagate_until_ev(hy_batch *b, const double *t_final_hi, const dou
                 HY_CUDA_CHECK(cudaMemcpyAsync(e.d_tf.get() + s.n, t_final_lo + off, sizeof(double) * s.n,
                                               cudaMemcpyHostToDevice, s.stream));
             }
-            e.ls = std::make_unique<lockstep>(s, e.d_tf.get(), t_final_lo != nullptr ? e.d_tf.get() + s.n : nullptr,
+            e.ls = std::make_shared<lockstep>(s, e.d_tf.get(), t_final_lo != nullptr ? e.d_tf.get() + s.n : nullptr,
                                               max_delta_t != nullptr ? max_delta_t + off : nullptr);
             e.ls->init();
             e.ls->read();
@@ -3051,86 +3146,31 @@ int hy_batch_propagate_grid_ev(hy_batch *b, const double *grid, uint64_t n_pts, 
         if (grid == nullptr || out == nullptr) {
             throw std::invalid_argument("Null pointer passed to hy_batch_propagate_grid_ev()");
         }
-        if (b->multi) {
-            throw hy::detail::not_implemented_error("propagate_grid() is not available on a multi-device batch");
-        }
         check_grid(b, grid, n_pts, max_delta_t);
-        shard &sh = *b->shards[0];
-        device_guard guard(sh.device);
-        const std::uint32_t n = sh.n;
-        const std::size_t n_out = static_cast<std::size_t>(n_pts) * sh.n_eq * n, state_doubles = std::size_t(sh.n_eq) * n;
-        const auto d_grid = dev_alloc<double>(n_pts * n), d_out = dev_alloc<double>(n_out);
-        const auto d_idx = dev_alloc<std::uint32_t>(n);
-        HY_CUDA_CHECK(cudaMemcpyAsync(d_grid.get(), grid, sizeof(double) * n_pts * n, cudaMemcpyHostToDevice, sh.stream));
-        dev::k_fill_double<<<static_cast<unsigned>((n_out + 255u) / 256u), 256, 0, sh.stream>>>(
-            d_out.get(), n_out, std::numeric_limits<double>::quiet_NaN());
-        HY_CUDA_CHECK(cudaGetLastError());
-        const unsigned gb = (n + 127u) / 128u;
-        const auto finish = [&]() {
-            HY_CUDA_CHECK(cudaMemcpyAsync(out, d_out.get(), sizeof(double) * n_out, cudaMemcpyDeviceToHost, sh.stream));
-            HY_CUDA_CHECK(cudaStreamSynchronize(sh.stream));
-            return HY_OK;
-        };
+        grid_run G(b, grid, n_pts, max_delta_t);
 
         // Up to the first grid point, with the events and their callbacks (:1697-1706: propagate_until()).
         ev_loop L(b, cb, user);
-        L.sh[0].ls = std::make_unique<lockstep>(sh, d_grid.get(), nullptr, max_delta_t);
-        L.sh[0].ls->init();
+        for_each_shard(b, [&](shard &s, std::size_t i) {
+            L.sh[i].ls = std::make_shared<lockstep>(s, G.p[i].d_grid.get(), nullptr, G.mdt(i));
+            L.sh[i].ls->init();
+        });
         L.run_until(max_steps, nullptr);
-        {
-            std::vector<long long> oc(n);
-            HY_CUDA_CHECK(cudaMemcpyAsync(oc.data(), sh.d_prop_outcome, sizeof(long long) * n, cudaMemcpyDeviceToHost,
-                                          sh.stream));
-            HY_CUDA_CHECK(cudaStreamSynchronize(sh.stream));
-            if (std::any_of(oc.begin(), oc.end(), [](long long v) { return v != HY_OUTCOME_TIME_LIMIT; })) {
-                // Outcomes kept, counters reset (:1709-1722).
-                dev::k_fill_double<<<gb, 128, 0, sh.stream>>>(sh.d_prop_min_h, n, std::numeric_limits<double>::infinity());
-                dev::k_fill_double<<<gb, 128, 0, sh.stream>>>(sh.d_prop_max_h, n, 0.);
-                HY_CUDA_CHECK(cudaMemsetAsync(sh.d_prop_n_steps, 0, sizeof(unsigned long long) * n, sh.stream));
-                return finish();
-            }
+        if (!G.first_leg_done()) {
+            return G.finish(out);
         }
-        HY_CUDA_CHECK(cudaMemcpyAsync(d_out.get(), sh.d_state, sizeof(double) * state_doubles, cudaMemcpyDeviceToDevice,
-                                      sh.stream));
-        // Grid point 0 is the state just copied: every cursor starts at 1.
-        const std::vector<std::uint32_t> first(n, 1u);
-        HY_CUDA_CHECK(cudaMemcpyAsync(d_idx.get(), first.data(), sizeof(std::uint32_t) * n, cudaMemcpyHostToDevice,
-                                      sh.stream));
 
         // Then the lock-step loop towards the last grid point, sampling after every iteration.
-        L.sh[0].ls = std::make_unique<lockstep>(sh, d_grid.get() + (n_pts - 1u) * n, nullptr, max_delta_t);
-        lockstep &ls = *L.sh[0].ls;
-        const dev::grid_state G{d_grid.get(), static_cast<std::uint32_t>(n_pts), d_out.get(), d_idx.get(),
-                                ls.d_flags.get() + 3};
-        const auto sample = [&](shard &s, std::size_t) {
-            dev::k_grid_sample<<<dim3(gb, s.n_eq), 128, 0, s.stream>>>(s.prog, s.view(), G, ls.L);
-            dev::k_grid_advance<<<gb, 128, 0, s.stream>>>(s.view(), G, ls.L);
-            HY_CUDA_CHECK(cudaGetLastError());
-        };
-        ls.init();
-        sample(sh, 0);
-        ls.read();
-        if (ls.flags[2] != 0u) {
-            throw std::invalid_argument("The final time passed to the propagate_grid() function of an adaptive Taylor "
-                                        "integrator in batch mode results in an overflow condition");
+        G.start(std::vector<const unsigned char *>(b->shards.size(), nullptr));
+        for (std::size_t i = 0; i < L.sh.size(); ++i) {
+            L.sh[i].ls = G.p[i].ls;
         }
-        L.iter = 0;
         L.stop = false;
-        bool interrupted = false;
-        while (ls.flags[3] != 0u && !interrupted) {
-            L.iterate(sample);
-            if (L.nf) {
-                break; // non-finite state: nothing further is written (:1973-1978)
-            }
-            // A stopping terminal event ends the loop once the grid points of this step are written.
-            interrupted = L.stop;
-            if (L.iter == max_steps) {
-                dev::k_fill_outcome<<<(n + 255u) / 256u, 256, 0, sh.stream>>>(sh.d_prop_outcome, n,
-                                                                              HY_OUTCOME_STEP_LIMIT);
-                interrupted = true;
-            }
-        }
-        return finish();
+        G.loop(max_steps, [&](const grid_run::shard_fn &hook) {
+            L.iterate(hook);
+            return L.stop;
+        });
+        return G.finish(out);
     } catch (const callback_abort &) {
         hy::detail::set_last_error("A host callback aborted the propagation");
         return HY_ERR_CALLBACK;

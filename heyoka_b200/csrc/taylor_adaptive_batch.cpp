@@ -1412,7 +1412,7 @@ taylor_adaptive_batch<double>::propagate_grid_impl(const std::vector<double> &gr
     }
     if (const auto *ar = o.cb ? o.cb.target<callback::angle_reducer>() : nullptr) {
         const auto idx = ar->get_sv_indices(*this); // (the reference's pre_hook(): before any step)
-        if (!with_events() && m.devices.empty() && device_reduces(m.batch)) {
+        if (!with_events() && device_reduces(m.batch)) {
             // The angle reducer on the device, inside the grid loop.
             const angle_scope scope(m.batch, idx);
             auto cb = std::move(o.cb);
@@ -1422,7 +1422,7 @@ taylor_adaptive_batch<double>::propagate_grid_impl(const std::vector<double> &gr
             return res;
         }
     }
-    if (!o.cb && with_events() && m.devices.empty()) {
+    if (!o.cb && with_events()) {
         // Events without a step callback: the lock-step loop on the device (hy_batch_propagate_grid_ev()).
         std::vector<double> retval(grid.size() * m.dim);
         m.push();
@@ -1438,10 +1438,9 @@ taylor_adaptive_batch<double>::propagate_grid_impl(const std::vector<double> &gr
         check(st);
         return {std::move(o.cb), std::move(retval)};
     }
-    if (o.cb || with_events() || !m.devices.empty()) {
-        // A step callback (or events, whose callbacks also run on the host) after every step: the reference's loop on the
-        // host, one device step per iteration. A batch sharded over several devices takes it too (the grid is sampled
-        // through the dense output of the shards).
+    if (o.cb || with_events()) {
+        // A step callback (with or without events, whose callbacks then run beside it) after every step: the
+        // reference's loop on the host, one device step per iteration.
         return propagate_grid_events(grid, std::move(o));
     }
     std::vector<double> retval(grid.size() * m.dim);

@@ -297,7 +297,8 @@ int hy_batch_propagate_until_host(hy_batch *, const double *state_in, const doub
  * grid[k * batch + lane], k < n_pts: finite, strictly monotonic with the same direction in every lane, and
  * grid[lane] == current time (hi part) of the lane. out[(k * n_eq + var) * batch + lane] receives the state at
  * grid point k; entries not reached (early exit: step limit, non-finite state) are NaN. The integrator ends at
- * the last grid point with outcome time_limit; results via hy_batch_download_prop_res(). host arrays. */
+ * the last grid point with outcome time_limit; results via hy_batch_download_prop_res(). host arrays. Any number of
+ * shards: they run the loop in lock-step and give the bits of the single-device batch. */
 int hy_batch_propagate_grid(hy_batch *, const double *grid, uint64_t n_pts, const double *max_delta_t,
                             uint64_t max_steps, double *out);
 
@@ -410,8 +411,8 @@ int hy_batch_set_cooldowns(hy_batch *, const uint8_t *active, const double *spen
  * at its target. The Taylor coefficients are always written. The angle reducer (hy_batch_set_angles()) is refused.
  * hy_batch_propagate_until_ev(): any number of shards; c_out (may be NULL) receives the continuous output of the call
  * (single device only), *c_out = NULL if no iteration completed. Results via hy_batch_download_prop_res().
- * hy_batch_propagate_grid_ev(): single device; the initial propagation to grid[0] runs the same loop with the same
- * callback; out[n_pts * n_eq * batch] as hy_batch_propagate_grid(). */
+ * hy_batch_propagate_grid_ev(): any number of shards; the initial propagation to grid[0] runs the same loop with the
+ * same callback; out[n_pts * n_eq * batch] as hy_batch_propagate_grid(). */
 typedef int (*hy_event_callback)(void *user, const hy_event_rec *recs, const double *t_hi, const double *t_lo,
                                  uint32_t n_rec, unsigned char *cont);
 int hy_batch_propagate_until_ev(hy_batch *, const double *t_final_hi, const double *t_final_lo,

@@ -58,6 +58,62 @@ def run(name, P, st, t_final=None, **kernel):
     print(json.dumps(res), flush=True)
 
 
+def grid_sharded():
+    """The "grid" workload (6-body, 16384 lanes x 1000 grid points over 20 yr, pinned output) on one device and on
+    sharded batches (two shards on device 0, and one shard per GPU when the box has several), through the C ABI. Then
+    the front end's host loop over the shards (forced by a step callback that returns True), on 2 yr and 100 grid points
+    because it runs per-lane Python loops at every iteration. Each line carries the card it ran on."""
+    import ctypes as C
+    import subprocess
+    card = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True,
+                          text=True).stdout.strip().splitlines()
+    batch, n_pts = 16384, 1000
+    P = hb.Program(sys_outer_ss(), high_accuracy=True)
+    st = outer_ss_batch_state(batch)
+    z = np.zeros(batch)
+    grid = np.ascontiguousarray(np.linspace(0., 20., n_pts)[:, None] * np.ones(batch)[None, :])
+    out = np.empty((n_pts, 36, batch))
+    dp = lambda a: a.ctypes.data_as(C.POINTER(C.c_double))  # noqa: E731
+    hb.check(hb.lib.hy_host_pin(C.c_void_p(out.ctypes.data), C.c_size_t(out.nbytes)))
+    n_dev = hb.lib.hy_device_count()
+    ref = None
+    for device in [-1, [0, 0]] + ([list(range(n_dev))] if n_dev > 1 else []):
+        b = hb.Batch(P, batch, device=device)
+        times = []
+        for _ in range(3):
+            b.upload(st, None, z, z)
+            b.sync()
+            l0 = b.launch_count()
+            t0 = time.perf_counter()
+            hb.check(hb.lib.hy_batch_propagate_grid(b._h, dp(grid), n_pts, None, 0, dp(out)))
+            times.append(time.perf_counter() - t0)
+            launches = b.launch_count() - l0
+        if ref is None:
+            ref = out.copy()
+        print(json.dumps({"config": "outer_ss 6-body propagate_grid, %d lanes x %d grid points over 20 yr" % (batch, n_pts),
+                          "device": device, "shards": max(b.n_shards, 1), "kernel": b.kernel_info()["tape"],
+                          "seconds": min(times), "seconds_all": times, "launches": int(launches),
+                          "readbacks_per_iteration": 1 if b.n_shards <= 1 else 2,
+                          "lane_steps": int(b.prop_res()[3].sum()),
+                          "same_bits_as_one_device": bool(np.array_equal(out.view(np.uint64), ref.view(np.uint64))),
+                          "card": card}), flush=True)
+        del b
+    hb.lib.hy_host_unpin(C.c_void_p(out.ctypes.data))
+    del out, ref
+    # The front end's host loop over the shards, as every sharded grid ran before it ran on the device.
+    span, pts = 2.0, 100
+    g = np.linspace(0., span, pts)[:, None] * np.ones(batch)[None, :]
+    for device, cb in (([0, 0], None), ([0, 0], lambda ta: True)):
+        ta = hb.taylor_adaptive_batch(sys_outer_ss(), st, batch, high_accuracy=True, device=device)
+        t0 = time.perf_counter()
+        ta.propagate_grid(g, callback=cb)
+        dt = time.perf_counter() - t0
+        print(json.dumps({"config": "outer_ss 6-body propagate_grid, %d lanes x %d grid points over %g yr, front end"
+                                    % (batch, pts, span), "device": device,
+                          "path": "device loop" if cb is None else "host loop (step callback)", "seconds": dt,
+                          "card": card}), flush=True)
+
+
 def main():
     which = sys.argv[1:] or ["tb", "n32", "nn", "s6step"]
     if "tbsmall" in which:
@@ -112,6 +168,8 @@ def main():
                           "seconds_pageable_output": res["pageable"], "launches": int(launches),
                           "lane_steps": int(b.prop_res()[3].sum()), "output_bytes": int(out.nbytes),
                           "output_gbs_incl_d2h": out.nbytes / res["pinned"] / 1e9}), flush=True)
+    if "gridshard" in which:
+        grid_sharded()
     if "n32" in which:
         st = nbody32_batch_state(8192)
         run("nbody N=32, 8192 lanes, propagate_until(1)", hb.Program(sys_nbody32()), st, 1.0)
