@@ -2295,10 +2295,9 @@ void check_grid(hy_batch *b, const double *grid, uint64_t n_pts, const double *m
     }
 }
 
-// The reference's lock-step loop (src/taylor_adaptive_batch.cpp:1372-1527, :1696-2053) as propagate_grid() and
-// propagate_until() with continuous output run it: the per-lane state of dev::lockstep_state and the buffers behind it.
-// An iteration is iterate(), whatever the caller launches after the bookkeeping, then read(): one read-back per
-// iteration.
+// The reference's lock-step loop (src/taylor_adaptive_batch.cpp:1372-1527, :1696-2053) on one shard: the per-lane state
+// of dev::lockstep_state and the buffers behind it. An iteration is a step (step(), or an event step), book(), whatever
+// the caller launches after the bookkeeping, then read(): one read-back per iteration.
 struct lockstep {
     shard &sh;
     dev_ptr<double> lane; // rem_hi, rem_lo, dt_limit, max_delta_t: [4][n]
@@ -2339,9 +2338,8 @@ struct lockstep {
                                                                 sh.d_prop_n_steps);
         HY_CUDA_CHECK(cudaGetLastError());
     }
-    // One step of every lane within its dt_limit, with its Taylor coefficients written to sh.d_tc, then the
-    // bookkeeping. All four flag words start the iteration cleared.
-    void iterate()
+    // One step of every lane within its dt_limit, with its Taylor coefficients written to sh.d_tc.
+    void step()
     {
         dev::run_args R{};
         R.max_delta_t = L.dt_limit;
@@ -2351,9 +2349,8 @@ struct lockstep {
         R.counter = sh.d_counter;
         R.angles = angles;
         sh.launch(false, R);
-        book();
     }
-    // The bookkeeping of the step just taken (an event step runs shard::ev_step(L.dt_limit, 0) and its callbacks first).
+    // The bookkeeping of the step just taken. All four flag words start it cleared.
     void book()
     {
         HY_CUDA_CHECK(cudaMemsetAsync(d_flags.get(), 0, sizeof(flags), sh.stream));
@@ -2388,157 +2385,6 @@ struct lockstep {
     }
 };
 
-// propagate_grid() on every shard of a batch: per shard its columns of the grid, its block of the output, its cursors
-// and the lock-step state of the loop towards the last grid point. The reference's loop runs over the whole batch, so
-// the shards run in lock-step: every shard takes every iteration while some lane of some shard has grid points left (a
-// shard whose lanes are all at their target takes zero-length steps, as those lanes do inside one device), and an
-// iteration in which a lane of any shard goes non-finite is sampled by no shard.
-struct grid_run {
-    struct part {
-        dev_ptr<double> d_grid, d_out; // [n_pts][n], [n_pts][n_eq][n]
-        dev_ptr<std::uint32_t> d_idx;
-        std::shared_ptr<lockstep> ls; // (shared with the event loop's shard state)
-    };
-    hy_batch *b;
-    std::uint64_t n_pts;
-    const double *max_delta_t;
-    std::vector<part> p; // one per shard of b
-
-    // Stages the grid by column and fills every shard's output with NaN.
-    grid_run(hy_batch *b_, const double *grid, std::uint64_t n_pts_, const double *max_delta_t_)
-        : b(b_), n_pts(n_pts_), max_delta_t(max_delta_t_), p(b_->shards.size())
-    {
-        for_each_shard(b, [&](shard &s, std::size_t i) {
-            const std::size_t n_out = static_cast<std::size_t>(n_pts) * s.n_eq * s.n;
-            p[i].d_grid = dev_alloc<double>(n_pts * s.n);
-            p[i].d_out = dev_alloc<double>(n_out);
-            p[i].d_idx = dev_alloc<std::uint32_t>(s.n);
-            rows_h2d(s, p[i].d_grid.get(), grid, n_pts, b->n, b->off[i]);
-            dev::k_fill_double<<<static_cast<unsigned>((n_out + 255u) / 256u), 256, 0, s.stream>>>(
-                p[i].d_out.get(), n_out, std::numeric_limits<double>::quiet_NaN());
-            HY_CUDA_CHECK(cudaGetLastError());
-            HY_CUDA_CHECK(cudaStreamSynchronize(s.stream));
-        });
-    }
-    const double *mdt(std::size_t i) const
-    {
-        return max_delta_t != nullptr ? max_delta_t + b->off[i] : nullptr;
-    }
-    // After the propagation to grid[0]: whether every lane of every shard reached it. If not, the counters are reset
-    // and the outcomes kept (:1709-1722).
-    bool first_leg_done()
-    {
-        std::vector<long long> oc(b->n);
-        for_each_shard(b, [&](shard &s, std::size_t i) {
-            rows_d2h(s, oc.data(), s.d_prop_outcome, 1u, b->n, b->off[i]);
-            HY_CUDA_CHECK(cudaStreamSynchronize(s.stream));
-        });
-        if (std::all_of(oc.begin(), oc.end(), [](long long v) { return v == HY_OUTCOME_TIME_LIMIT; })) {
-            return true;
-        }
-        for_each_shard(b, [&](shard &s, std::size_t) {
-            const unsigned gb = (s.n + 127u) / 128u;
-            dev::k_fill_double<<<gb, 128, 0, s.stream>>>(s.d_prop_min_h, s.n, std::numeric_limits<double>::infinity());
-            dev::k_fill_double<<<gb, 128, 0, s.stream>>>(s.d_prop_max_h, s.n, 0.);
-            HY_CUDA_CHECK(cudaGetLastError());
-            HY_CUDA_CHECK(cudaMemsetAsync(s.d_prop_n_steps, 0, sizeof(unsigned long long) * s.n, s.stream));
-            HY_CUDA_CHECK(cudaStreamSynchronize(s.stream));
-        });
-        return false;
-    }
-    // Grid point 0 is the current state, every cursor starts at 1; the lock-step states towards the last grid point
-    // (each shard's reduced rows: angles[i]), and the grid points the zero-length interval before the first step covers.
-    void start(const std::vector<const unsigned char *> &angles)
-    {
-        for_each_shard(b, [&](shard &s, std::size_t i) {
-            part &q = p[i];
-            HY_CUDA_CHECK(cudaMemcpyAsync(q.d_out.get(), s.d_state, sizeof(double) * s.n_eq * s.n,
-                                          cudaMemcpyDeviceToDevice, s.stream));
-            const std::vector<std::uint32_t> first(s.n, 1u);
-            HY_CUDA_CHECK(cudaMemcpyAsync(q.d_idx.get(), first.data(), sizeof(std::uint32_t) * s.n,
-                                          cudaMemcpyHostToDevice, s.stream));
-            q.ls = std::make_shared<lockstep>(s, q.d_grid.get() + (n_pts - 1u) * s.n, nullptr, mdt(i));
-            q.ls->angles = angles[i];
-            q.ls->init();
-            sample(s, i);
-            q.ls->read();
-        });
-        for (const auto &q : p) {
-            if (q.ls->flags[2] != 0u) {
-                throw std::invalid_argument("The final time passed to the propagate_grid() function of an adaptive "
-                                            "Taylor integrator in batch mode results in an overflow condition");
-            }
-        }
-    }
-    // Dense output at the grid points the shard's last step covered, and the cursors past them. The word the lock-step
-    // state leaves to its caller is set when some lane has grid points left.
-    void sample(shard &s, std::size_t i)
-    {
-        const part &q = p[i];
-        const dev::grid_state G{q.d_grid.get(), static_cast<std::uint32_t>(n_pts), q.d_out.get(), q.d_idx.get(),
-                                q.ls->d_flags.get() + 3};
-        const unsigned gb = q.ls->blocks();
-        dev::k_grid_sample<<<dim3(gb, s.n_eq), 128, 0, s.stream>>>(s.prog, s.view(), G, q.ls->L);
-        dev::k_grid_advance<<<gb, 128, 0, s.stream>>>(s.view(), G, q.ls->L);
-        HY_CUDA_CHECK(cudaGetLastError());
-    }
-    bool any_flag(unsigned w) const
-    {
-        return std::any_of(p.begin(), p.end(), [w](const part &q) { return q.ls->flags[w] != 0u; });
-    }
-    // The lock-step loop (:1770-2053). iterate(hook) takes one iteration on every shard - step, bookkeeping, then
-    // hook(shard, i), then the flags read back - and returns true when it must be the last one (a stopping terminal
-    // event). One shard samples inside the hook, where the kernels' own check of the non-finite flag is batch-wide: one
-    // read-back per iteration. More shards combine their non-finite flags on the host first, then sample and read the
-    // flags again.
-    using shard_fn = std::function<void(shard &, std::size_t)>;
-    void loop(std::uint64_t max_steps, const std::function<bool(const shard_fn &)> &iterate)
-    {
-        const bool one = p.size() == 1u;
-        const shard_fn hook = [&](shard &s, std::size_t i) {
-            if (one) {
-                sample(s, i);
-            }
-        };
-        std::uint64_t iter = 0;
-        while (any_flag(3)) {
-            const bool stop = iterate(hook);
-            if (any_flag(1)) {
-                // Non-finite state: nothing further is written, and the reduction of this step is undone (:1973-1978).
-                for_each_shard(b, [&](shard &, std::size_t i) { p[i].ls->undo_reduction(); });
-                return;
-            }
-            if (!one) {
-                for_each_shard(b, [&](shard &s, std::size_t i) {
-                    sample(s, i);
-                    p[i].ls->read();
-                });
-            }
-            if (++iter == max_steps) {
-                for_each_shard(b, [&](shard &s, std::size_t) {
-                    dev::k_fill_outcome<<<(s.n + 255u) / 256u, 256, 0, s.stream>>>(s.d_prop_outcome, s.n,
-                                                                                    HY_OUTCOME_STEP_LIMIT);
-                    HY_CUDA_CHECK(cudaGetLastError());
-                    HY_CUDA_CHECK(cudaStreamSynchronize(s.stream));
-                });
-                return;
-            }
-            if (stop) {
-                return; // once the grid points of this step are written
-            }
-        }
-    }
-    // Every shard's block of the output into the caller's [n_pts][n_eq][batch] array.
-    int finish(double *out)
-    {
-        for_each_shard(b, [&](shard &s, std::size_t i) {
-            rows_d2h(s, out, p[i].d_out.get(), static_cast<std::size_t>(n_pts) * s.n_eq, b->n, b->off[i]);
-            HY_CUDA_CHECK(cudaStreamSynchronize(s.stream));
-        });
-        return HY_OK;
-    }
-};
-
 } // namespace
 
 int hy_batch_check_grid(hy_batch *b, const double *grid, uint64_t n_pts, const double *max_delta_t)
@@ -2549,42 +2395,6 @@ int hy_batch_check_grid(hy_batch *b, const double *grid, uint64_t n_pts, const d
         }
         check_grid(b, grid, n_pts, max_delta_t);
         return HY_OK;
-    } catch (...) {
-        return translate_exception();
-    }
-}
-
-int hy_batch_propagate_grid(hy_batch *b, const double *grid, uint64_t n_pts, const double *max_delta_t,
-                            uint64_t max_steps, double *out)
-{
-    try {
-        refuse_events(b);
-        if (b == nullptr || grid == nullptr || out == nullptr) {
-            throw std::invalid_argument("Null pointer passed to hy_batch_propagate_grid()");
-        }
-        check_grid(b, grid, n_pts, max_delta_t);
-        std::vector<const unsigned char *> angles(b->shards.size());
-        for (std::size_t i = 0; i < b->shards.size(); ++i) {
-            angles[i] = b->shards[i]->prop_angles();
-        }
-        grid_run G(b, grid, n_pts, max_delta_t);
-
-        // Up to the first grid point (a zero-length step when the time is already there: it brings the Taylor
-        // coefficients up to date), :1697-1706. The reference calls no step callback there: no reduction.
-        propagate(b, grid, nullptr, max_delta_t, 0, max_steps, 1, nullptr, false);
-        if (!G.first_leg_done()) {
-            return G.finish(out);
-        }
-        G.start(angles);
-        G.loop(max_steps, [&](const grid_run::shard_fn &hook) {
-            for_each_shard(b, [&](shard &s, std::size_t i) {
-                G.p[i].ls->iterate();
-                hook(s, i);
-                G.p[i].ls->read();
-            });
-            return false;
-        });
-        return G.finish(out);
     } catch (...) {
         return translate_exception();
     }
@@ -2609,9 +2419,9 @@ struct hy_cout {
 
 // A recording under construction (update_c_out() / make_c_out(), src/taylor_adaptive_batch.cpp:1277-1346): the
 // Taylor coefficients of the current iteration go to slot(), commit() appends the times and closes the iteration.
-// The device loop of hy_batch_propagate_until_cout_cb() has the step kernel write straight into the slot; the front
-// ends' host lock-step loops (integrators with events, whose callbacks are host code) copy the step's tc array there
-// through hy_cout_rec_append().
+// Plain steps of the device lock-step loop have the step kernel write straight into the slot; append() copies the
+// batch's tc array there first, for event steps (on the device, and in the front ends' host lock-step loops through
+// hy_cout_rec_append()).
 struct hy_cout_rec {
     std::unique_ptr<hy_cout> co;
     dev_ptr<double> d_times; // rows of 2 * n doubles (hi, lo)
@@ -2621,6 +2431,7 @@ struct hy_cout_rec {
     explicit hy_cout_rec(shard &sh);
     double *slot();
     void commit(shard &sh);
+    void append(shard &sh);
     hy_cout *finish(shard &sh, const unsigned char *forward);
 
 private:
@@ -2678,6 +2489,13 @@ void hy_cout_rec::commit(shard &sh)
     ++iter;
 }
 
+// (The rows of the state variables come first in the batch's tc array; those of event equations are not recorded.)
+void hy_cout_rec::append(shard &sh)
+{
+    HY_CUDA_CHECK(cudaMemcpyAsync(slot(), sh.d_tc, sizeof(double) * tc_doubles, cudaMemcpyDeviceToDevice, sh.stream));
+    commit(sh);
+}
+
 // make_c_out() (:1277-1317): forward[lane] != 0 for lanes integrated forwards in time (the padding row of the times is
 // +-inf by direction). Null if nothing was recorded.
 hy_cout *hy_cout_rec::finish(shard &sh, const unsigned char *forward)
@@ -2711,109 +2529,6 @@ hy_cout *hy_cout_rec::finish(shard &sh, const unsigned char *forward)
     return co.release();
 }
 
-namespace
-{
-struct callback_abort {
-};
-} // namespace
-
-int hy_batch_propagate_until_cout(hy_batch *b, const double *t_final_hi, const double *t_final_lo,
-                                  const double *max_delta_t, uint64_t max_steps, hy_cout **out)
-{
-    return hy_batch_propagate_until_cout_cb(b, t_final_hi, t_final_lo, max_delta_t, max_steps, nullptr, nullptr, out);
-}
-
-int hy_batch_propagate_until_cout_cb(hy_batch *b, const double *t_final_hi, const double *t_final_lo,
-                                     const double *max_delta_t, uint64_t max_steps, hy_step_callback cb, void *user,
-                                     hy_cout **out)
-{
-    try {
-        refuse_events(b);
-        if (b != nullptr && b->multi) {
-            throw hy::detail::not_implemented_error("Continuous output is not available on a multi-device batch");
-        }
-        if (b == nullptr || t_final_hi == nullptr || out == nullptr) {
-            throw std::invalid_argument("Null pointer passed to hy_batch_propagate_until_cout()");
-        }
-        *out = nullptr;
-        shard &sh = *b->shards[0];
-        device_guard guard(sh.device);
-        const std::uint32_t n = sh.n;
-        check_prop_args(n, t_final_hi, t_final_lo, max_delta_t);
-        const auto d_tf = dev_alloc<double>(2u * std::size_t(n)); // tf_hi, tf_lo
-        HY_CUDA_CHECK(cudaMemcpyAsync(d_tf.get(), t_final_hi, sizeof(double) * n, cudaMemcpyHostToDevice, sh.stream));
-        if (t_final_lo != nullptr) {
-            HY_CUDA_CHECK(cudaMemcpyAsync(d_tf.get() + n, t_final_lo, sizeof(double) * n, cudaMemcpyHostToDevice,
-                                          sh.stream));
-        }
-        lockstep ls(sh, d_tf.get(), t_final_lo != nullptr ? d_tf.get() + n : nullptr, max_delta_t);
-        ls.angles = sh.prop_angles();
-        hy_cout_rec rec(sh);
-        // The step kernel writes the coefficients of every iteration straight into their slot of the recording; the
-        // batch's own tc array is put back however the loop ends.
-        sh.ensure_tc();
-        struct tc_restore {
-            shard &sh;
-            double *const own;
-            ~tc_restore()
-            {
-                sh.d_tc = own;
-            }
-        } tc{sh, sh.d_tc};
-        ls.init();
-        ls.read();
-        if (ls.flags[2] != 0u) {
-            throw std::invalid_argument("The final time passed to the propagate_until() function of an adaptive "
-                                        "Taylor integrator in batch mode results in an overflow condition");
-        }
-        while (true) {
-            sh.d_tc = rec.slot();
-            ls.iterate();
-            ls.read();
-            if (ls.flags[1] != 0u) {
-                ls.undo_reduction();
-                break; // non-finite state: this iteration is not recorded (:1462-1467)
-            }
-            rec.commit(sh); // update_c_out(), :1320-1346
-            if (cb != nullptr) {
-                // The step callback (:1476-1500), before the exit tests like in the reference.
-                HY_CUDA_CHECK(cudaStreamSynchronize(sh.stream));
-                const int r = cb(user);
-                if (r < 0) {
-                    throw callback_abort{};
-                }
-                if (r == 0) {
-                    dev::k_fill_outcome<<<(n + 255u) / 256u, 256, 0, sh.stream>>>(sh.d_prop_outcome, n,
-                                                                                  HY_OUTCOME_CB_STOP);
-                    break;
-                }
-            }
-            if (ls.flags[0] == n) {
-                break; // every lane reached its final time
-            }
-            if (rec.iter == max_steps) {
-                dev::k_fill_outcome<<<(n + 255u) / 256u, 256, 0, sh.stream>>>(sh.d_prop_outcome, n,
-                                                                              HY_OUTCOME_STEP_LIMIT);
-                break;
-            }
-        }
-        // The batch's own tc array ends up with the coefficients of the last step taken, like m_tc in the reference.
-        HY_CUDA_CHECK(cudaMemcpyAsync(tc.own, sh.d_tc, sizeof(double) * rec.tc_doubles, cudaMemcpyDeviceToDevice,
-                                      sh.stream));
-        std::vector<unsigned char> forward(n);
-        HY_CUDA_CHECK(cudaMemcpyAsync(forward.data(), ls.L.t_dir, n, cudaMemcpyDeviceToHost, sh.stream));
-        HY_CUDA_CHECK(cudaStreamSynchronize(sh.stream));
-        *out = rec.finish(sh, forward.data());
-        HY_CUDA_CHECK(cudaStreamSynchronize(sh.stream));
-        return HY_OK;
-    } catch (const callback_abort &) {
-        hy::detail::set_last_error("A host callback aborted the propagation");
-        return HY_ERR_CALLBACK;
-    } catch (...) {
-        return translate_exception();
-    }
-}
-
 int hy_cout_rec_begin(hy_batch *b, hy_cout_rec **out)
 {
     try {
@@ -2845,10 +2560,7 @@ int hy_cout_rec_append(hy_batch *b, hy_cout_rec *r)
         }
         shard &sh = *b->shards[0];
         device_guard guard(sh.device);
-        // (The rows of the state variables come first in the batch's tc array; those of event equations are not recorded.)
-        HY_CUDA_CHECK(cudaMemcpyAsync(r->slot(), sh.d_tc, sizeof(double) * r->tc_doubles, cudaMemcpyDeviceToDevice,
-                                      sh.stream));
-        r->commit(sh);
+        r->append(sh);
         return HY_OK;
     } catch (...) {
         return translate_exception();
@@ -2880,38 +2592,45 @@ int hy_cout_rec_finish(hy_batch *b, hy_cout_rec *rp, const unsigned char *forwar
 }
 
 // ------------------------------------------------------------------------------------------------
-// Propagation of a batch with event equations (hy_batch_propagate_until_ev(), hy_batch_propagate_grid_ev()): the
-// reference's lock-step loop (src/taylor_adaptive_batch.cpp:1372-1527, :1696-2053) over event steps, with the
-// bookkeeping on the device. The host takes part in an iteration only when some lane produced an event record: it
-// receives the records with their absolute times and hands back the terminal-event decisions.
+// The lock-step propagations: propagate_until() with continuous output (hy_batch_propagate_until_cout{,_cb}()),
+// propagate_grid() (hy_batch_propagate_grid()), and both for a batch with event equations
+// (hy_batch_propagate_until_ev(), hy_batch_propagate_grid_ev()). One driver runs the reference's lock-step loop
+// (src/taylor_adaptive_batch.cpp:1372-1527, :1696-2053) over the shards of a batch, with the bookkeeping on the device.
+// A batch with events takes event steps: the host takes part in an iteration only when some lane produced an event
+// record, receives the records with their absolute times and hands back the terminal-event decisions.
 // ------------------------------------------------------------------------------------------------
 namespace
 {
 
-struct ev_shard {
-    std::shared_ptr<lockstep> ls;
-    dev_ptr<double> d_tf;          // target times of propagate_until() (hi, lo)
-    std::vector<hy_event_rec> recs; // live records of the iteration, lanes local to the shard
-    std::vector<double> t;          // their absolute times: [2][recs.size()] (hi, lo)
-    std::vector<std::uint32_t> go;  // local lanes whose terminal-event callback continues
-    dev_ptr<unsigned char> d_buf;   // staging of records, times and lanes
-    std::size_t buf_bytes = 0;
-
-    unsigned char *buf(std::size_t bytes)
-    {
-        if (bytes > buf_bytes) {
-            buf_bytes = std::max(bytes, 2u * buf_bytes);
-            d_buf = dev_alloc<unsigned char>(buf_bytes);
-        }
-        return d_buf.get();
-    }
+struct callback_abort {
 };
 
-struct ev_loop {
+// The lock-step loop over every shard of a batch. The reference's loop runs over the whole batch, so the shards run in
+// lock-step and the loop's exits are decided from the flags of all of them. cb == null: plain steps (lockstep::step());
+// otherwise event steps, with cb the events' callback.
+struct lockstep_run {
+    struct part {
+        std::unique_ptr<lockstep> ls;
+        dev_ptr<double> d_tf;           // target times of propagate_until() (hi, lo)
+        std::vector<hy_event_rec> recs; // live records of the iteration, lanes local to the shard
+        std::vector<double> t;          // their absolute times: [2][recs.size()] (hi, lo)
+        std::vector<std::uint32_t> go;  // local lanes whose terminal-event callback continues
+        dev_ptr<unsigned char> d_buf;   // staging of records, times and lanes
+        std::size_t buf_bytes = 0;
+
+        unsigned char *buf(std::size_t bytes)
+        {
+            if (bytes > buf_bytes) {
+                buf_bytes = std::max(bytes, 2u * buf_bytes);
+                d_buf = dev_alloc<unsigned char>(buf_bytes);
+            }
+            return d_buf.get();
+        }
+    };
     hy_batch *b;
     hy_event_callback cb;
     void *user;
-    std::vector<ev_shard> sh; // one per shard of b
+    std::vector<part> sh; // one per shard of b
     std::vector<hy_event_rec> recs;
     std::vector<double> t_hi, t_lo;
     std::vector<unsigned char> cont;
@@ -2921,14 +2640,47 @@ struct ev_loop {
     bool nf = false;        // a lane went non-finite in the last iteration
     bool stop = false;      // a terminal event without a callback, or whose callback returned false, fired
 
-    ev_loop(hy_batch *b_, hy_event_callback cb_, void *user_) : b(b_), cb(cb_), user(user_), sh(b_->shards.size()) {}
+    lockstep_run(hy_batch *b_, hy_event_callback cb_, void *user_) : b(b_), cb(cb_), user(user_), sh(b_->shards.size()) {}
 
-    // One iteration of every shard: event step, callbacks (if there are records), terminal-event decisions,
-    // bookkeeping, then after_book(shard, i) and the flags read back.
-    void iterate(const std::function<void(shard &, std::size_t)> &after_book)
+    // The lock-step states towards per-lane final times (host arrays; t_final_lo and max_delta_t may be null), with
+    // each shard's reduced rows.
+    void until(const double *t_final_hi, const double *t_final_lo, const double *max_delta_t)
     {
         for_each_shard(b, [&](shard &s, std::size_t i) {
-            ev_shard &e = sh[i];
+            const std::size_t off = b->off[i];
+            part &e = sh[i];
+            e.d_tf = dev_alloc<double>(2u * std::size_t(s.n));
+            HY_CUDA_CHECK(cudaMemcpyAsync(e.d_tf.get(), t_final_hi + off, sizeof(double) * s.n, cudaMemcpyHostToDevice,
+                                          s.stream));
+            if (t_final_lo != nullptr) {
+                HY_CUDA_CHECK(cudaMemcpyAsync(e.d_tf.get() + s.n, t_final_lo + off, sizeof(double) * s.n,
+                                              cudaMemcpyHostToDevice, s.stream));
+            }
+            e.ls = std::make_unique<lockstep>(s, e.d_tf.get(), t_final_lo != nullptr ? e.d_tf.get() + s.n : nullptr,
+                                              max_delta_t != nullptr ? max_delta_t + off : nullptr);
+            e.ls->angles = s.prop_angles();
+            e.ls->init();
+            e.ls->read();
+        });
+        check_overflow("propagate_until()");
+    }
+    // After init() and read(): the remaining time of every lane must be representable. fn names the caller.
+    void check_overflow(const char *fn) const
+    {
+        for (const auto &e : sh) {
+            if (e.ls->flags[2] != 0u) {
+                throw std::invalid_argument(std::string("The final time passed to the ") + fn
+                                            + " function of an adaptive Taylor integrator in batch mode results in an "
+                                              "overflow condition");
+            }
+        }
+    }
+
+    // The event step of every shard, then the callbacks (if there are records) and the terminal-event decisions.
+    void event_step()
+    {
+        for_each_shard(b, [&](shard &s, std::size_t i) {
+            part &e = sh[i];
             e.recs = s.ev_step(e.ls->L.dt_limit, 0);
             const auto k = static_cast<std::uint32_t>(e.recs.size());
             e.t.resize(2u * std::size_t(k));
@@ -2959,52 +2711,68 @@ struct ev_loop {
                 t_lo.push_back(sh[i].t[k + j]);
             }
         }
-        if (!recs.empty()) {
-            cont.assign(recs.size(), 0u);
-            const int r = cb(user, recs.data(), t_hi.data(), t_lo.data(), static_cast<std::uint32_t>(recs.size()),
-                             cont.data());
-            std::size_t k = 0;
-            for (auto &e : sh) {
-                e.go.clear();
-                for (const auto &rec : e.recs) {
-                    if (rec.terminal != 0) {
-                        if (cont[k] != 0u) {
-                            e.go.push_back(rec.lane);
-                        } else {
-                            stop = true;
-                        }
+        if (recs.empty()) {
+            return;
+        }
+        cont.assign(recs.size(), 0u);
+        const int r = cb(user, recs.data(), t_hi.data(), t_lo.data(), static_cast<std::uint32_t>(recs.size()),
+                         cont.data());
+        std::size_t k = 0;
+        for (auto &e : sh) {
+            e.go.clear();
+            for (const auto &rec : e.recs) {
+                if (rec.terminal != 0) {
+                    if (cont[k] != 0u) {
+                        e.go.push_back(rec.lane);
+                    } else {
+                        stop = true;
                     }
-                    ++k;
                 }
-            }
-            // The decisions are applied whatever the callback returned, like the front ends' loops do lane by lane.
-            for_each_shard(b, [&](shard &s, std::size_t i) {
-                ev_shard &e = sh[i];
-                const auto n_go = static_cast<std::uint32_t>(e.go.size());
-                if (n_go != 0u) {
-                    auto *d_lanes = reinterpret_cast<std::uint32_t *>(e.buf(sizeof(std::uint32_t) * n_go));
-                    HY_CUDA_CHECK(cudaMemcpyAsync(d_lanes, e.go.data(), sizeof(std::uint32_t) * n_go,
-                                                  cudaMemcpyHostToDevice, s.stream));
-                    dev::k_ev_continue<<<(n_go + 127u) / 128u, 128, 0, s.stream>>>(s.view(), d_lanes, n_go);
-                    HY_CUDA_CHECK(cudaGetLastError());
-                    ++s.n_launches;
-                }
-                if (r < 0 && !started) {
-                    // Aborted before any bookkeeping: the per-lane results read as before the first step.
-                    dev::k_fill_outcome<<<(s.n + 255u) / 256u, 256, 0, s.stream>>>(s.d_prop_outcome, s.n, 0);
-                    dev::k_fill_double<<<(s.n + 255u) / 256u, 256, 0, s.stream>>>(s.d_prop_min_h, s.n, 0.);
-                    HY_CUDA_CHECK(cudaGetLastError());
-                }
-                HY_CUDA_CHECK(cudaStreamSynchronize(s.stream));
-            });
-            if (r < 0) {
-                throw callback_abort{};
+                ++k;
             }
         }
+        // The decisions are applied whatever the callback returned, like the front ends' loops do lane by lane.
         for_each_shard(b, [&](shard &s, std::size_t i) {
-            sh[i].ls->book();
-            after_book(s, i);
-            sh[i].ls->read();
+            part &e = sh[i];
+            const auto n_go = static_cast<std::uint32_t>(e.go.size());
+            if (n_go != 0u) {
+                auto *d_lanes = reinterpret_cast<std::uint32_t *>(e.buf(sizeof(std::uint32_t) * n_go));
+                HY_CUDA_CHECK(cudaMemcpyAsync(d_lanes, e.go.data(), sizeof(std::uint32_t) * n_go,
+                                              cudaMemcpyHostToDevice, s.stream));
+                dev::k_ev_continue<<<(n_go + 127u) / 128u, 128, 0, s.stream>>>(s.view(), d_lanes, n_go);
+                HY_CUDA_CHECK(cudaGetLastError());
+                ++s.n_launches;
+            }
+            if (r < 0 && !started) {
+                // Aborted before any bookkeeping: the per-lane results read as before the first step.
+                dev::k_fill_outcome<<<(s.n + 255u) / 256u, 256, 0, s.stream>>>(s.d_prop_outcome, s.n, 0);
+                dev::k_fill_double<<<(s.n + 255u) / 256u, 256, 0, s.stream>>>(s.d_prop_min_h, s.n, 0.);
+                HY_CUDA_CHECK(cudaGetLastError());
+            }
+            HY_CUDA_CHECK(cudaStreamSynchronize(s.stream));
+        });
+        if (r < 0) {
+            throw callback_abort{};
+        }
+    }
+
+    // One iteration of every shard: the step, the bookkeeping, then after_book(shard, i) if given and the flags read
+    // back.
+    void iterate(const std::function<void(shard &, std::size_t)> &after_book = nullptr)
+    {
+        if (cb != nullptr) {
+            event_step();
+        }
+        for_each_shard(b, [&](shard &s, std::size_t i) {
+            lockstep &ls = *sh[i].ls;
+            if (cb == nullptr) {
+                ls.step();
+            }
+            ls.book();
+            if (after_book) {
+                after_book(s, i);
+            }
+            ls.read();
         });
         started = true;
         done = 0u;
@@ -3015,41 +2783,247 @@ struct ev_loop {
         }
         ++iter;
     }
-    void iterate()
+
+    void undo_reduction()
     {
-        iterate([](shard &, std::size_t) {});
+        for_each_shard(b, [&](shard &, std::size_t i) { sh[i].ls->undo_reduction(); });
     }
 
-    // propagate_until() from the lock-step states already initialised: iterations up to the loop's exits, every
-    // iteration that ends with finite states recorded by rec (single shard, on the shard's device) if given.
-    void run_until(std::uint64_t max_steps, hy_cout_rec *rec)
+    void fill_outcome(long long oc)
+    {
+        for_each_shard(b, [&](shard &s, std::size_t) {
+            dev::k_fill_outcome<<<(s.n + 255u) / 256u, 256, 0, s.stream>>>(s.d_prop_outcome, s.n, oc);
+            HY_CUDA_CHECK(cudaGetLastError());
+            HY_CUDA_CHECK(cudaStreamSynchronize(s.stream));
+        });
+    }
+
+    // propagate_until() from the lock-step states already initialised: iterations up to the loop's exits, in the
+    // reference's order. Every iteration that ends with finite states is recorded by rec (shard 0's recorder) if given,
+    // and followed by the step callback step_cb(step_user) if given.
+    void run_until(std::uint64_t max_steps, hy_cout_rec *rec, hy_step_callback step_cb, void *step_user)
     {
         shard &s0 = *b->shards[0];
+        // Plain steps record in place: the step kernel writes the coefficients of every iteration straight into their
+        // slot of the recording (a copy would move the whole tc array once per iteration), and the batch's own tc array
+        // is put back however the loop ends. The tc array of an event step also holds the event rows: it is copied.
+        // (The recorder allocates its slabs and times on shard 0's device.)
+        const bool in_place = rec != nullptr && cb == nullptr;
+        if (in_place) {
+            device_guard guard(s0.device);
+            s0.ensure_tc();
+        }
+        struct tc_restore {
+            shard &sh;
+            double *const own; // null: nothing to put back
+            ~tc_restore()
+            {
+                if (own != nullptr) {
+                    sh.d_tc = own;
+                }
+            }
+        } tc{s0, in_place ? s0.d_tc : nullptr};
         while (true) {
+            if (in_place) {
+                device_guard guard(s0.device);
+                s0.d_tc = rec->slot();
+            }
             iterate();
             if (nf) {
-                return; // non-finite state: this iteration is not recorded (:1462-1467)
+                undo_reduction();
+                break; // non-finite state: this iteration is not recorded (:1462-1467)
             }
             if (rec != nullptr) {
-                // (The recorder allocates its slabs and times on the shard's device.)
+                // update_c_out(), :1320-1346
                 device_guard guard(s0.device);
-                HY_CUDA_CHECK(cudaMemcpyAsync(rec->slot(), s0.d_tc, sizeof(double) * rec->tc_doubles,
-                                              cudaMemcpyDeviceToDevice, s0.stream));
-                rec->commit(s0);
+                if (in_place) {
+                    rec->commit(s0);
+                } else {
+                    rec->append(s0);
+                }
+            }
+            if (step_cb != nullptr) {
+                // The step callback (:1476-1500), before the exit tests like in the reference.
+                HY_CUDA_CHECK(cudaStreamSynchronize(s0.stream));
+                const int r = step_cb(step_user);
+                if (r < 0) {
+                    throw callback_abort{};
+                }
+                if (r == 0) {
+                    fill_outcome(HY_OUTCOME_CB_STOP);
+                    break;
+                }
             }
             if (stop || done == b->n) {
-                return;
+                break; // a stopping terminal event, or every lane reached its final time
             }
             if (iter == max_steps) {
-                for_each_shard(b, [&](shard &s, std::size_t) {
-                    dev::k_fill_outcome<<<(s.n + 255u) / 256u, 256, 0, s.stream>>>(s.d_prop_outcome, s.n,
-                                                                                    HY_OUTCOME_STEP_LIMIT);
-                    HY_CUDA_CHECK(cudaGetLastError());
-                    HY_CUDA_CHECK(cudaStreamSynchronize(s.stream));
-                });
-                return;
+                fill_outcome(HY_OUTCOME_STEP_LIMIT);
+                break;
             }
         }
+        if (in_place) {
+            // The batch's own tc array ends up with the coefficients of the last step taken, like m_tc in the reference.
+            device_guard guard(s0.device);
+            HY_CUDA_CHECK(cudaMemcpyAsync(tc.own, s0.d_tc, sizeof(double) * rec->tc_doubles, cudaMemcpyDeviceToDevice,
+                                          s0.stream));
+        }
+    }
+};
+
+// propagate_grid() on every shard of a batch: per shard its columns of the grid, its block of the output and its
+// cursors, and the driver L with the lock-step states towards the last grid point. Every shard takes every iteration
+// while some lane of some shard has grid points left (a shard whose lanes are all at their target takes zero-length
+// steps, as those lanes do inside one device), and an iteration in which a lane of any shard goes non-finite is
+// sampled by no shard.
+struct grid_run {
+    struct part {
+        dev_ptr<double> d_grid, d_out; // [n_pts][n], [n_pts][n_eq][n]
+        dev_ptr<std::uint32_t> d_idx;
+    };
+    hy_batch *b;
+    std::uint64_t n_pts;
+    const double *max_delta_t;
+    std::vector<part> p; // one per shard of b
+    lockstep_run L;
+
+    // Stages the grid by column and fills every shard's output with NaN.
+    grid_run(hy_batch *b_, const double *grid, std::uint64_t n_pts_, const double *max_delta_t_, hy_event_callback cb,
+             void *user)
+        : b(b_), n_pts(n_pts_), max_delta_t(max_delta_t_), p(b_->shards.size()), L(b_, cb, user)
+    {
+        for_each_shard(b, [&](shard &s, std::size_t i) {
+            const std::size_t n_out = static_cast<std::size_t>(n_pts) * s.n_eq * s.n;
+            p[i].d_grid = dev_alloc<double>(n_pts * s.n);
+            p[i].d_out = dev_alloc<double>(n_out);
+            p[i].d_idx = dev_alloc<std::uint32_t>(s.n);
+            rows_h2d(s, p[i].d_grid.get(), grid, n_pts, b->n, b->off[i]);
+            dev::k_fill_double<<<static_cast<unsigned>((n_out + 255u) / 256u), 256, 0, s.stream>>>(
+                p[i].d_out.get(), n_out, std::numeric_limits<double>::quiet_NaN());
+            HY_CUDA_CHECK(cudaGetLastError());
+            HY_CUDA_CHECK(cudaStreamSynchronize(s.stream));
+        });
+    }
+    const double *mdt(std::size_t i) const
+    {
+        return max_delta_t != nullptr ? max_delta_t + b->off[i] : nullptr;
+    }
+    // Up to the first grid point (:1697-1706: propagate_until(grid[0])).
+    void first_leg(const double *grid, std::uint64_t max_steps)
+    {
+        if (L.cb == nullptr) {
+            // A zero-length step when the time is already there: it brings the Taylor coefficients up to date. The
+            // reference calls no step callback there: no reduction.
+            propagate(b, grid, nullptr, max_delta_t, 0, max_steps, 1, nullptr, false);
+            return;
+        }
+        // With the events and their callbacks.
+        for_each_shard(b, [&](shard &s, std::size_t i) {
+            L.sh[i].ls = std::make_unique<lockstep>(s, p[i].d_grid.get(), nullptr, mdt(i));
+            L.sh[i].ls->init();
+        });
+        L.run_until(max_steps, nullptr, nullptr, nullptr);
+    }
+    // After the propagation to grid[0]: whether every lane of every shard reached it. If not, the counters are reset
+    // and the outcomes kept (:1709-1722).
+    bool first_leg_done()
+    {
+        std::vector<long long> oc(b->n);
+        for_each_shard(b, [&](shard &s, std::size_t i) {
+            rows_d2h(s, oc.data(), s.d_prop_outcome, 1u, b->n, b->off[i]);
+            HY_CUDA_CHECK(cudaStreamSynchronize(s.stream));
+        });
+        if (std::all_of(oc.begin(), oc.end(), [](long long v) { return v == HY_OUTCOME_TIME_LIMIT; })) {
+            return true;
+        }
+        for_each_shard(b, [&](shard &s, std::size_t) {
+            const unsigned gb = (s.n + 127u) / 128u;
+            dev::k_fill_double<<<gb, 128, 0, s.stream>>>(s.d_prop_min_h, s.n, std::numeric_limits<double>::infinity());
+            dev::k_fill_double<<<gb, 128, 0, s.stream>>>(s.d_prop_max_h, s.n, 0.);
+            HY_CUDA_CHECK(cudaGetLastError());
+            HY_CUDA_CHECK(cudaMemsetAsync(s.d_prop_n_steps, 0, sizeof(unsigned long long) * s.n, s.stream));
+            HY_CUDA_CHECK(cudaStreamSynchronize(s.stream));
+        });
+        return false;
+    }
+    // Grid point 0 is the current state, every cursor starts at 1; the lock-step states towards the last grid point
+    // (each shard's reduced rows: angles[i]), and the grid points the zero-length interval before the first step covers.
+    void start(const std::vector<const unsigned char *> &angles)
+    {
+        for_each_shard(b, [&](shard &s, std::size_t i) {
+            part &q = p[i];
+            HY_CUDA_CHECK(cudaMemcpyAsync(q.d_out.get(), s.d_state, sizeof(double) * s.n_eq * s.n,
+                                          cudaMemcpyDeviceToDevice, s.stream));
+            const std::vector<std::uint32_t> first(s.n, 1u);
+            HY_CUDA_CHECK(cudaMemcpyAsync(q.d_idx.get(), first.data(), sizeof(std::uint32_t) * s.n,
+                                          cudaMemcpyHostToDevice, s.stream));
+            L.sh[i].ls = std::make_unique<lockstep>(s, q.d_grid.get() + (n_pts - 1u) * s.n, nullptr, mdt(i));
+            L.sh[i].ls->angles = angles[i];
+            L.sh[i].ls->init();
+            sample(s, i);
+            L.sh[i].ls->read();
+        });
+        L.check_overflow("propagate_grid()");
+    }
+    // Dense output at the grid points the shard's last step covered, and the cursors past them. The word the lock-step
+    // state leaves to its caller is set when some lane has grid points left.
+    void sample(shard &s, std::size_t i)
+    {
+        const part &q = p[i];
+        const lockstep &ls = *L.sh[i].ls;
+        const dev::grid_state G{q.d_grid.get(), static_cast<std::uint32_t>(n_pts), q.d_out.get(), q.d_idx.get(),
+                                ls.d_flags.get() + 3};
+        const unsigned gb = ls.blocks();
+        dev::k_grid_sample<<<dim3(gb, s.n_eq), 128, 0, s.stream>>>(s.prog, s.view(), G, ls.L);
+        dev::k_grid_advance<<<gb, 128, 0, s.stream>>>(s.view(), G, ls.L);
+        HY_CUDA_CHECK(cudaGetLastError());
+    }
+    bool any_flag(unsigned w) const
+    {
+        return std::any_of(L.sh.begin(), L.sh.end(), [w](const lockstep_run::part &e) { return e.ls->flags[w] != 0u; });
+    }
+    // The lock-step loop (:1770-2053). One shard samples right after its bookkeeping, where the kernels' own check of
+    // the non-finite flag is batch-wide: one read-back per iteration. More shards combine their non-finite flags on the
+    // host first, then sample and read the flags again.
+    void loop(std::uint64_t max_steps)
+    {
+        const bool one = p.size() == 1u;
+        L.stop = false;
+        std::uint64_t iter = 0;
+        while (any_flag(3)) {
+            L.iterate([&](shard &s, std::size_t i) {
+                if (one) {
+                    sample(s, i);
+                }
+            });
+            if (L.nf) {
+                // Non-finite state: nothing further is written, and the reduction of this step is undone (:1973-1978).
+                L.undo_reduction();
+                return;
+            }
+            if (!one) {
+                for_each_shard(b, [&](shard &s, std::size_t i) {
+                    sample(s, i);
+                    L.sh[i].ls->read();
+                });
+            }
+            if (++iter == max_steps) {
+                L.fill_outcome(HY_OUTCOME_STEP_LIMIT);
+                return;
+            }
+            if (L.stop) {
+                return; // a stopping terminal event, once the grid points of this step are written
+            }
+        }
+    }
+    // Every shard's block of the output into the caller's [n_pts][n_eq][batch] array.
+    int finish(double *out)
+    {
+        for_each_shard(b, [&](shard &s, std::size_t i) {
+            rows_d2h(s, out, p[i].d_out.get(), static_cast<std::size_t>(n_pts) * s.n_eq, b->n, b->off[i]);
+            HY_CUDA_CHECK(cudaStreamSynchronize(s.stream));
+        });
+        return HY_OK;
     }
 };
 
@@ -3073,7 +3047,91 @@ void check_ev_batch(const hy_batch *b, hy_event_callback cb, const char *fn)
     }
 }
 
+// propagate_until() of every lane of a checked batch: event steps with the events' callback cb, or plain steps with the
+// step callback step_cb (either may be null; user goes to the one given), recorded into *c_out if c_out is not null.
+int propagate_until_lockstep(hy_batch *b, const double *t_final_hi, const double *t_final_lo,
+                             const double *max_delta_t, uint64_t max_steps, hy_event_callback cb,
+                             hy_step_callback step_cb, void *user, hy_cout **c_out)
+{
+    try {
+        lockstep_run L(b, cb, user);
+        L.until(t_final_hi, t_final_lo, max_delta_t);
+        shard &s0 = *b->shards[0];
+        std::unique_ptr<hy_cout_rec> rec;
+        if (c_out != nullptr) {
+            device_guard guard(s0.device);
+            rec = std::make_unique<hy_cout_rec>(s0);
+        }
+        L.run_until(max_steps, rec.get(), step_cb, user);
+        if (rec != nullptr) {
+            device_guard guard(s0.device);
+            std::vector<unsigned char> forward(s0.n);
+            HY_CUDA_CHECK(cudaMemcpyAsync(forward.data(), L.sh[0].ls->L.t_dir, s0.n, cudaMemcpyDeviceToHost, s0.stream));
+            HY_CUDA_CHECK(cudaStreamSynchronize(s0.stream));
+            *c_out = rec->finish(s0, forward.data());
+            HY_CUDA_CHECK(cudaStreamSynchronize(s0.stream));
+        }
+        return HY_OK;
+    } catch (const callback_abort &) {
+        hy::detail::set_last_error("A host callback aborted the propagation");
+        return HY_ERR_CALLBACK;
+    }
+}
+
+// propagate_grid() of every lane of a checked batch: event steps with the events' callback cb, or plain steps with the
+// angle reducer.
+int propagate_grid_lockstep(hy_batch *b, const double *grid, uint64_t n_pts, const double *max_delta_t,
+                            uint64_t max_steps, hy_event_callback cb, void *user, double *out)
+{
+    try {
+        // (Before any grid work: a refused angle list leaves the batch untouched. Event batches have none.)
+        std::vector<const unsigned char *> angles(b->shards.size());
+        for (std::size_t i = 0; i < b->shards.size(); ++i) {
+            angles[i] = b->shards[i]->prop_angles();
+        }
+        grid_run G(b, grid, n_pts, max_delta_t, cb, user);
+        G.first_leg(grid, max_steps);
+        if (!G.first_leg_done()) {
+            return G.finish(out);
+        }
+        G.start(angles);
+        G.loop(max_steps);
+        return G.finish(out);
+    } catch (const callback_abort &) {
+        hy::detail::set_last_error("A host callback aborted the propagation");
+        return HY_ERR_CALLBACK;
+    }
+}
+
 } // namespace
+
+int hy_batch_propagate_until_cout(hy_batch *b, const double *t_final_hi, const double *t_final_lo,
+                                  const double *max_delta_t, uint64_t max_steps, hy_cout **out)
+{
+    return hy_batch_propagate_until_cout_cb(b, t_final_hi, t_final_lo, max_delta_t, max_steps, nullptr, nullptr, out);
+}
+
+int hy_batch_propagate_until_cout_cb(hy_batch *b, const double *t_final_hi, const double *t_final_lo,
+                                     const double *max_delta_t, uint64_t max_steps, hy_step_callback cb, void *user,
+                                     hy_cout **out)
+{
+    try {
+        refuse_events(b);
+        if (b != nullptr && b->multi) {
+            throw hy::detail::not_implemented_error("Continuous output is not available on a multi-device batch");
+        }
+        if (b == nullptr || t_final_hi == nullptr || out == nullptr) {
+            throw std::invalid_argument("Null pointer passed to hy_batch_propagate_until_cout()");
+        }
+        *out = nullptr;
+        // (The step callback runs with the batch's device current.)
+        device_guard guard(b->shards[0]->device);
+        check_prop_args(b->n, t_final_hi, t_final_lo, max_delta_t);
+        return propagate_until_lockstep(b, t_final_hi, t_final_lo, max_delta_t, max_steps, nullptr, cb, user, out);
+    } catch (...) {
+        return translate_exception();
+    }
+}
 
 int hy_batch_propagate_until_ev(hy_batch *b, const double *t_final_hi, const double *t_final_lo,
                                 const double *max_delta_t, uint64_t max_steps, hy_event_callback cb, void *user,
@@ -3092,47 +3150,22 @@ int hy_batch_propagate_until_ev(hy_batch *b, const double *t_final_hi, const dou
         }
         check_prop_args(b->n, t_final_hi, t_final_lo, max_delta_t);
         check_prop_times(b, t_final_hi, t_final_lo);
-        ev_loop L(b, cb, user);
-        for_each_shard(b, [&](shard &s, std::size_t i) {
-            const std::size_t off = b->off[i];
-            ev_shard &e = L.sh[i];
-            e.d_tf = dev_alloc<double>(2u * std::size_t(s.n));
-            HY_CUDA_CHECK(cudaMemcpyAsync(e.d_tf.get(), t_final_hi + off, sizeof(double) * s.n, cudaMemcpyHostToDevice,
-                                          s.stream));
-            if (t_final_lo != nullptr) {
-                HY_CUDA_CHECK(cudaMemcpyAsync(e.d_tf.get() + s.n, t_final_lo + off, sizeof(double) * s.n,
-                                              cudaMemcpyHostToDevice, s.stream));
-            }
-            e.ls = std::make_shared<lockstep>(s, e.d_tf.get(), t_final_lo != nullptr ? e.d_tf.get() + s.n : nullptr,
-                                              max_delta_t != nullptr ? max_delta_t + off : nullptr);
-            e.ls->init();
-            e.ls->read();
-        });
-        for (const auto &e : L.sh) {
-            if (e.ls->flags[2] != 0u) {
-                throw std::invalid_argument("The final time passed to the propagate_until() function of an adaptive "
-                                            "Taylor integrator in batch mode results in an overflow condition");
-            }
+        return propagate_until_lockstep(b, t_final_hi, t_final_lo, max_delta_t, max_steps, cb, nullptr, user, c_out);
+    } catch (...) {
+        return translate_exception();
+    }
+}
+
+int hy_batch_propagate_grid(hy_batch *b, const double *grid, uint64_t n_pts, const double *max_delta_t,
+                            uint64_t max_steps, double *out)
+{
+    try {
+        refuse_events(b);
+        if (b == nullptr || grid == nullptr || out == nullptr) {
+            throw std::invalid_argument("Null pointer passed to hy_batch_propagate_grid()");
         }
-        shard &s0 = *b->shards[0];
-        std::unique_ptr<hy_cout_rec> rec;
-        if (c_out != nullptr) {
-            device_guard guard(s0.device);
-            rec = std::make_unique<hy_cout_rec>(s0);
-        }
-        L.run_until(max_steps, rec.get());
-        if (rec != nullptr) {
-            device_guard guard(s0.device);
-            std::vector<unsigned char> forward(s0.n);
-            HY_CUDA_CHECK(cudaMemcpyAsync(forward.data(), L.sh[0].ls->L.t_dir, s0.n, cudaMemcpyDeviceToHost, s0.stream));
-            HY_CUDA_CHECK(cudaStreamSynchronize(s0.stream));
-            *c_out = rec->finish(s0, forward.data());
-            HY_CUDA_CHECK(cudaStreamSynchronize(s0.stream));
-        }
-        return HY_OK;
-    } catch (const callback_abort &) {
-        hy::detail::set_last_error("A host callback aborted the propagation");
-        return HY_ERR_CALLBACK;
+        check_grid(b, grid, n_pts, max_delta_t);
+        return propagate_grid_lockstep(b, grid, n_pts, max_delta_t, max_steps, nullptr, nullptr, out);
     } catch (...) {
         return translate_exception();
     }
@@ -3147,33 +3180,7 @@ int hy_batch_propagate_grid_ev(hy_batch *b, const double *grid, uint64_t n_pts, 
             throw std::invalid_argument("Null pointer passed to hy_batch_propagate_grid_ev()");
         }
         check_grid(b, grid, n_pts, max_delta_t);
-        grid_run G(b, grid, n_pts, max_delta_t);
-
-        // Up to the first grid point, with the events and their callbacks (:1697-1706: propagate_until()).
-        ev_loop L(b, cb, user);
-        for_each_shard(b, [&](shard &s, std::size_t i) {
-            L.sh[i].ls = std::make_shared<lockstep>(s, G.p[i].d_grid.get(), nullptr, G.mdt(i));
-            L.sh[i].ls->init();
-        });
-        L.run_until(max_steps, nullptr);
-        if (!G.first_leg_done()) {
-            return G.finish(out);
-        }
-
-        // Then the lock-step loop towards the last grid point, sampling after every iteration.
-        G.start(std::vector<const unsigned char *>(b->shards.size(), nullptr));
-        for (std::size_t i = 0; i < L.sh.size(); ++i) {
-            L.sh[i].ls = G.p[i].ls;
-        }
-        L.stop = false;
-        G.loop(max_steps, [&](const grid_run::shard_fn &hook) {
-            L.iterate(hook);
-            return L.stop;
-        });
-        return G.finish(out);
-    } catch (const callback_abort &) {
-        hy::detail::set_last_error("A host callback aborted the propagation");
-        return HY_ERR_CALLBACK;
+        return propagate_grid_lockstep(b, grid, n_pts, max_delta_t, max_steps, cb, user, out);
     } catch (...) {
         return translate_exception();
     }
